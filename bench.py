@@ -1,13 +1,15 @@
 """Benchmark of the denoise hot path (BASELINE.json metric: TSP-500 graphs/sec, 50-step categorical).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
 A "step" = one pass of the hot path over one batch: the full 50-step categorical denoise of
 16 TSP-500 (k=50) instances batched block-diagonally in one call (BASELINE config[1]), per GPU.
 Weak scaling: every rank owns its own batch; no collective inside the loop; for N > 1 the final
 heatmaps are all-gathered over NCCL inside the timed region (north_star).
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  --dump-outputs DIR writes the heat map the last timed step returned
+(DIR/heatmap.npy, float32, caller edge order; all ranks' maps concatenated for N > 1).  Inputs, weights and
+sampling seeds are fixed, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -41,7 +43,7 @@ def workload_config(n_gpus):
           "nodes_per_graph": N_NODES, "knn": KNN, "batch_per_gpu": BATCH, "denoise_steps": DENOISE_STEPS,
           "global_batch": BATCH * n_gpus, "parallelism": f"dp{n_gpus} (independent batches, no in-loop collective)",
           "weights": "seeded random init of the reference architecture (12 layers, hidden 256), per_layer_out de-zeroed",
-          "l2_policy": "working set (edge stream 410 MB/GPU) exceeds the 126 MB L2; no explicit flush needed"}
+          "l2_policy": "working set (edge stream 410 MB/GPU) exceeds the 50 MB L2; no explicit flush needed"}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -94,19 +96,7 @@ def measured_peaks():
   if os.path.exists(p):
     d = json.load(open(p))
     return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, sustained copy)"
-  return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic():
-  """dram__bytes_read.sum + dram__bytes_write.sum of ALL launches of one denoise step of the headline workload, from the
-  committed ncu pass (profiles/r02_step_traffic.json; same scope as roofline.achieved: the whole step)."""
-  p = os.path.join(ROOT, "profiles", "r02_step_traffic.json")
-  if os.path.exists(p):
-    try:
-      return json.load(open(p)).get("dram_bytes_per_step")
-    except Exception:
-      return None
-  return None
+  return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -276,7 +266,7 @@ def run_reference(args, rank, world):
 
 # ------------------------------------------------------------------------------------------------
 # BASELINE.json configs.  configs[1] (C2) is the headline workload the default run times; --config C1|C3|C4|C5 time the
-# other ones through the same code path and print the same JSON schema (profiles/r02_other_configs.jsonl).
+# other ones through the same code path and print the same JSON schema.
 CONFIGS = {
     "C1": dict(task="tsp", nodes=50, knn=-1, batch=1, diffusion="categorical",
                label="TSP-50 dense graph, categorical diffusion, 1 instance, 50 denoise steps (BASELINE configs[0])"),
@@ -405,10 +395,13 @@ def run_ours(args, rank, world, local_rank):
   if world > 1:
     dist.all_reduce(ms, op=dist.ReduceOp.MAX)
   total_ms = float(ms.item())
-  hm = x.cpu().numpy()
+  hm = torch.cat(gathered).cpu().numpy() if world > 1 else x.cpu().numpy()
   assert np.isfinite(hm).all()
   if categorical:
     assert hm.min() >= 0.0 and hm.max() <= 1.0 + 1e-5
+  if args.dump_outputs and rank == 0:
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    np.save(os.path.join(args.dump_outputs, "heatmap.npy"), hm.astype(np.float32))
 
   # ---- the dominant kernel on its own: ONE more batch with per-launch CUDA events on the launching stream (plain
   #      launches: events cannot be recorded inside the captured graph the timed region replays); not part of `value`
@@ -462,19 +455,18 @@ def run_ours(args, rank, world, local_rank):
       wlc["workload"] = cfg["label"] + ", per GPU"
       wlc.update(nodes_per_graph=cfg["nodes"], knn=cfg["knn"], batch_per_gpu=cfg["batch"], global_batch=cfg["batch"] * world)
       wlc["l2_policy"] = (f"edge stream {E * H * 4 / 1e6:.0f} MB per GPU" +
-                          (" exceeds the 126 MB L2" if E * H * 4 > 126e6 else " fits the 126 MB L2 (no flush: the loop streams it 24x per step)"))
+                          (" exceeds the 50 MB L2" if E * H * 4 > 50e6 else " fits the 50 MB L2 (no flush: the loop streams it 24x per step)"))
     line = {"metric": METRIC if args.config == "C2" else f"{args.config} graphs/sec, 50-step denoise ({cfg['label']})",
             "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": total_ms / args.steps, "higher_is_better": True,
-            "scaling": "weak", "vs_baseline": None, "dtype": "f32 (3-term bf16 split on tcgen05, fp32 accumulate)",
+            "scaling": "weak", "vs_baseline": None, "dtype": "f32 (3-term bf16 split on wgmma, fp32 accumulate)",
             "data": "synthetic", "config": wlc,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": ncu_traffic(), "peak_source": peak_src,
+                         "peak_source": peak_src,
                          "scope": "whole denoise step: every launch of the timed loop (CUDA-graph replay), timed with CUDA "
                                   "events around the loop; algorithmic bytes = SURVEY 8(d) per step",
                          "algorithmic_bytes_per_step": step_bytes, "denoise_steps_timed": DENOISE_STEPS * args.steps,
-                         "kernel": {"name": "k_edge_layer_pair (CTA-pair fused edge layer, all 12 layers; layer 0 in table-lookup "
-                                            "mode without the input read; the MIS last layer: k_edge_layer_tc16w)"
+                         "kernel": {"name": "k_edge_layer_wg2 (fused edge layer, two wgmma warpgroups per CTA, all 12 layers)"
                                     if impl == "tc" else impl,
                                     "algorithmic_bytes_per_launch": per_launch_bytes, "launches_timed": int(edge_n),
                                     "ms_per_launch": k_ms, "achieved": k_achieved, "frac": k_achieved / peak,
@@ -513,6 +505,8 @@ def main():
   ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
   ap.add_argument("--config", default="C2", choices=sorted(CONFIGS), help="BASELINE.json config (default C2 = configs[1], the headline)")
   ap.add_argument("--no-cpu-baseline", dest="no_cpu_baseline", action="store_true")
+  ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                  help="write the heat map of the last timed step to DIR/heatmap.npy (float32)")
   args = ap.parse_args()
   rank = int(os.environ.get("RANK", "0"))
   world = int(os.environ.get("WORLD_SIZE", "1"))

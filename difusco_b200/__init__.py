@@ -1,4 +1,4 @@
-"""difusco_b200: B200-native (sm_100a) implementation of DIFUSCO's denoising-inference hot path.
+"""difusco_b200: H100-native (sm_90a) implementation of DIFUSCO's denoising-inference hot path.
 
 Host mirror of the reference interface (same module / class / method names):
     difusco_b200.models.gnn_encoder.GNNEncoder

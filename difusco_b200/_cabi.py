@@ -1,5 +1,5 @@
 """ctypes binding of include/difusco_b200.h.  The ONLY compute backend: if the shared library is
-missing or no B200 is present every call fails loudly - there is no eager/CPU fallback."""
+missing or no H100 is present every call fails loudly - there is no eager/CPU fallback."""
 import ctypes as C
 import os
 

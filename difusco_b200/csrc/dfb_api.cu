@@ -14,7 +14,6 @@
 #include "common.cuh"
 #include "edge_layer_fp32.cuh"
 #include "edge_layer_tc.cuh"
-#include "edge_layer_v2.cuh"
 #include "kernels_small.cuh"
 #include "knn.cuh"
 #include "tsp_decode.cuh"
@@ -48,7 +47,6 @@ struct dfb_ctx {
   bool graph_ready = false, points_ready = false;
   GraphDev g{};
   int gn_segments = 1;
-  int max_seg = 0;   // most node segments inside one 32-edge group (pair kernel handles up to v2::MAXSEG)
   DevBuf d_row, d_col, d_perm, d_rowptr, d_grp_first, d_grp_pair, d_ei_stage;
   // ---- workspace ----
   DevBuf e, h, h0, uvab, uvab0, partials, feat, tvec, tvals, gn_part, gn_stats, d_points, d_xt, d_u;
@@ -73,11 +71,11 @@ struct dfb_ctx {
   cudaEvent_t loop_in = nullptr, loop_out = nullptr;   // legacy default stream, which cannot be captured), fenced by events
   struct LoopKey {
     uint64_t buf_gen = ~0ull;
-    int steps = 0, diffusion = 0, impl = 0, agg = 0, pair = 0;
+    int steps = 0, diffusion = 0, impl = 0, agg = 0;
     const void* uniforms = nullptr;
     bool operator==(const LoopKey& o) const {
       return buf_gen == o.buf_gen && steps == o.steps && diffusion == o.diffusion && impl == o.impl && agg == o.agg &&
-             pair == o.pair && uniforms == o.uniforms;
+             uniforms == o.uniforms;
     }
   } loop_key;
   int64_t loop_launches = 0;     // kernel launches inside one replay of the captured loop
@@ -87,9 +85,6 @@ struct dfb_ctx {
   std::vector<cudaEvent_t> ev_pool;
   size_t ev_used = 0;
   TcState tc;
-  v2::State pair;   // round-2 CTA-pair kernel (middle layers of the product path)
-  bool pair_enabled = true;    // DFB_PAIR_KERNEL=0 routes every layer to the single-CTA kernel (A/B timing)
-  bool serpentine = true;      // DFB_SERPENTINE=0: every layer sweeps the edge stream upwards (A/B timing)
 };
 
 #define FAIL(ctx, code, ...)                         \
@@ -177,9 +172,9 @@ extern "C" int dfb_create(dfb_ctx** out, int device) {
   }
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, device);
-  if (prop.major != 10) {
+  if (prop.major != 9 || prop.minor != 0) {
     char b[160];
-    snprintf(b, sizeof(b), "device %d is sm_%d%d; this library is built for sm_100a (B200) only", device,
+    snprintf(b, sizeof(b), "device %d is sm_%d%d; this library is built for sm_90a (H100) only", device,
              prop.major, prop.minor);
     g_create_error = b;
     return DFB_E_UNSUPPORTED;
@@ -194,7 +189,7 @@ extern "C" int dfb_create(dfb_ctx** out, int device) {
   }
   int r = tc_init(&ctx->tc, prop.multiProcessorCount);
   if (r != 0) {
-    g_create_error = "tcgen05 edge kernel setup failed: " + ctx->tc.err;
+    g_create_error = "tensor-core edge kernel setup failed: " + ctx->tc.err;
     delete ctx;
     return DFB_E_CUDA;
   }
@@ -217,18 +212,6 @@ extern "C" int dfb_create(dfb_ctx** out, int device) {
   {
     const char* cg = getenv("DFB_GRAPH_CAPTURE");
     if (cg && atoi(cg) == 0) ctx->capture_enabled = false;
-  }
-  {
-    const char* pk = getenv("DFB_PAIR_KERNEL");
-    if (pk) ctx->pair_enabled = atoi(pk) != 0;
-    const char* sp = getenv("DFB_SERPENTINE");
-    if (sp) ctx->serpentine = atoi(sp) != 0;
-  }
-  r = v2::init(&ctx->pair, &ctx->tc);
-  if (r != 0) {
-    g_create_error = "tcgen05 pair kernel setup failed: " + ctx->tc.err;
-    delete ctx;
-    return DFB_E_CUDA;
   }
   *out = ctx;
   return DFB_OK;
@@ -464,8 +447,6 @@ extern "C" int dfb_load_weights(dfb_ctx* ctx, int n_layers, int hidden_dim, int 
 
   int r = tc_bind_weights(&ctx->tc, ctx->layers.data(), L);
   if (r) FAIL(ctx, DFB_E_CUDA, "tensor-map setup failed: %s", ctx->tc.err.c_str());
-  r = v2::bind_weights(&ctx->pair, &ctx->tc, ctx->wbuf16.p, L);
-  if (r) FAIL(ctx, DFB_E_CUDA, "tensor-map setup failed: %s", ctx->tc.err.c_str());
 
   // categorical edge-embedding LUT: edge_embed(edge_pos_embed(x)) for x in {0, 1}
   if (!node_feature_only) {
@@ -550,17 +531,13 @@ extern "C" int dfb_prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_
   }
   const int nG = (E + GROUP - 1) / GROUP;
   std::vector<int> gfirst(nG), gpair((size_t)nG + 1);
-  int np = 0, max_seg = 0;
+  int np = 0;
   for (int gI = 0; gI < nG; ++gI) {
     int s0 = gI * GROUP, s1 = std::min(E, s0 + GROUP) - 1;
     gfirst[gI] = row[s0];
     gpair[gI] = np;
     np += row[s1] - row[s0] + 1;
-    int segs = 1;
-    for (int q = s0 + 1; q <= s1; ++q) segs += row[q] != row[q - 1];
-    max_seg = std::max(max_seg, segs);
   }
-  ctx->max_seg = max_seg;
   gpair[nG] = np;
 
   ENS(ctx, ctx->d_row, (size_t)E * 4);
@@ -588,11 +565,7 @@ extern "C" int dfb_prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_
   ctx->gn_segments = gn_segments;
 
   // workspace
-  const size_t Epad = (size_t)((E + 127) / 128) * 128;   // whole 128-row tiles for the tensor-core kernel
-  ENS(ctx, ctx->e, Epad * H * sizeof(float));
-  // the padding rows of the last tile are carried through every layer like real rows (and discarded): they must start
-  // finite, or a stale NaN would travel with them
-  if (Epad > (size_t)E) CK(ctx, cudaMemsetAsync((float*)ctx->e.p + (size_t)E * H, 0, (Epad - E) * H * sizeof(float), st));
+  ENS(ctx, ctx->e, (size_t)E * H * sizeof(float));
   ENS(ctx, ctx->h, (size_t)V * H * sizeof(float));
   ENS(ctx, ctx->h0, (size_t)V * H * sizeof(float));
   ENS(ctx, ctx->uvab, (size_t)V * 4 * H * sizeof(float));
@@ -623,7 +596,7 @@ static int node_linears(dfb_ctx* ctx, int l, const float* h, float* uvab, int V,
     return DFB_OK;
   }
   int r = tc_launch_linear(&ctx->tc, l * 12 * H + 4 * H, 4, h, uvab, ctx->layers[l].b_uvab, V, ctx->g, ctx->layers[l], st);
-  if (r) FAIL(ctx, DFB_E_CUDA, "tcgen05 node linear: %s", ctx->tc.err.c_str());
+  if (r) FAIL(ctx, DFB_E_CUDA, "tensor-core node linear: %s", ctx->tc.err.c_str());
   ctx->launches += 1;
   return DFB_OK;
 }
@@ -644,7 +617,7 @@ static int embed_rows(dfb_ctx* ctx, int which, const float* X, float* Y, int R, 
     return linear_rows(ctx, X, which ? ctx->Wt_node : ctx->Wt_edge, which ? ctx->b_node : ctx->b_edge, Y, R, H, st);
   int r = tc_launch_linear(&ctx->tc, (ctx->L * 12 + 2 * which) * H, 1, X, Y, which ? ctx->b_node : ctx->b_edge, R, ctx->g,
                            ctx->layers[0], st);
-  if (r) FAIL(ctx, DFB_E_CUDA, "tcgen05 embedding linear: %s", ctx->tc.err.c_str());
+  if (r) FAIL(ctx, DFB_E_CUDA, "tensor-core embedding linear: %s", ctx->tc.err.c_str());
   ctx->launches += 1;
   return DFB_OK;
 }
@@ -680,10 +653,8 @@ extern "C" int dfb_set_points(dfb_ctx* ctx, const float* points, void* stream_) 
 // ================================================================================================
 // one forward (+ optional fused posterior)
 // ================================================================================================
-// gn_blocks: when non-null and the pair kernel runs this layer, it also produces the head's GroupNorm partial sums
-// (ctx->gn_part) and *gn_blocks receives the number of partial blocks; otherwise *gn_blocks stays 0.
 static int launch_edge_layer(dfb_ctx* ctx, int l, const float* uvab, const float* tvec_edge, int write_e,
-                             int e_zero, const float* xt_for_lut, cudaStream_t st, int* gn_blocks = nullptr) {
+                             int e_zero, const float* xt_for_lut, cudaStream_t st) {
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   if (ctx->profiling) {
     if (ctx->ev_used + 2 > ctx->ev_pool.size()) {
@@ -707,26 +678,11 @@ static int launch_edge_layer(dfb_ctx* ctx, int l, const float* uvab, const float
                                                             ctx->g, ctx->layers[l], tvec_edge, write_e,
                                                             ctx->agg_mode);
     CKL(ctx);
-  } else if (ctx->edge_impl == DFB_EDGE_IMPL_TC && ctx->pair_enabled && ctx->max_seg <= v2::MAXSEG && write_e &&
-             (!(e_zero || xt_for_lut) || ctx->L > 1)) {
-    // the CTA-pair kernel: middle layers read and write the edge stream; layer 0 (table rows in, SURVEY D5) runs in LUT mode
-    const bool lut_mode = e_zero || xt_for_lut;
-    const float* cl = lut_mode ? (e_zero ? ctx->cl0 + 2 * H : ctx->cl0) : nullptr;       // e0 = 0: zero tables
-    const float* lut = lut_mode ? (e_zero ? ctx->cl0 + 2 * H : ctx->lut) : nullptr;
-    // the last layer that writes e (TSP: L-1, read next by the head from row 0 up; MIS: L-2, read by the last layer's
-    // kernel from tile 0 up) sweeps the edge stream downwards, the one before it upwards, and so on
-    const int last_writer = ctx->node_only ? ctx->L - 2 : ctx->L - 1;
-    const int sweep_down = (((last_writer - l) & 1) == 0 && l <= last_writer && ctx->serpentine) ? 1 : 0;
-    int r = v2::launch(&ctx->pair, &ctx->tc, l, (float*)ctx->e.p, uvab, (float*)ctx->partials.p, ctx->g, ctx->layers[l],
-                       tvec_edge, ctx->agg_mode, st, gn_blocks ? (double*)ctx->gn_part.p : nullptr, gn_blocks,
-                       xt_for_lut, cl, lut, sweep_down);
-    if (r) FAIL(ctx, DFB_E_CUDA, "tcgen05 pair edge layer: %s", ctx->tc.err.c_str());
-    ctx->launches += ctx->tc.last_launches;
   } else {
     int r = tc_launch_edge_layer(&ctx->tc, l, (float*)ctx->e.p, uvab, (float*)ctx->partials.p, ctx->g,
                                  ctx->layers[l], tvec_edge, write_e, e_zero, xt_for_lut, ctx->lut,
-                                 ctx->agg_mode, st);
-    if (r) FAIL(ctx, r == -3 ? DFB_E_UNSUPPORTED : DFB_E_CUDA, "tcgen05 edge layer: %s", ctx->tc.err.c_str());
+                                 ctx->agg_mode, st, ctx->edge_impl == DFB_EDGE_IMPL_TC1 ? 1 : 2);
+    if (r) FAIL(ctx, DFB_E_CUDA, "tensor-core edge layer: %s", ctx->tc.err.c_str());
     ctx->launches += ctx->tc.last_launches;
   }
   if (ctx->profiling) CK(ctx, cudaEventRecord(ev1, st));
@@ -771,7 +727,6 @@ static int run_forward(dfb_ctx* ctx, const float* xt, const float* tvec, bool bi
     }
     e_zero = 1;   // gnn_encoder.py:407: e0 = zeros
   }
-  int gn_fused_blocks = 0;
   for (int l = 0; l < L; ++l) {
     const float* uv = uvab;
     if (l == 0 && !ctx->node_only) {
@@ -782,10 +737,8 @@ static int run_forward(dfb_ctx* ctx, const float* xt, const float* tvec, bool bi
     }
     const float* tv = tvec + (size_t)l * H;
     int write_e = !(ctx->node_only && l == L - 1);
-    // the last layer of the sparse TSP encoder also accumulates the head's GroupNorm statistics (one segment only)
-    const bool want_gn = !ctx->node_only && l == L - 1 && ctx->gn_segments == 1;
     int r = launch_edge_layer(ctx, l, uv, ctx->node_only ? nullptr : tv, write_e, (l == 0) ? e_zero : 0,
-                              (l == 0) ? xt_lut : nullptr, st, want_gn ? &gn_fused_blocks : nullptr);
+                              (l == 0) ? xt_lut : nullptr, st);
     if (r) return r;
     if (ctx->node_only || l < L - 1) {   // TSP never reads h after the last layer (gnn_encoder.py:400)
       k_node_update<<<(V + 7) / 8, 256, 0, st>>>(h, uv, (const float*)ctx->partials.p, g, ctx->layers[l].ln_h_g,
@@ -798,15 +751,10 @@ static int run_forward(dfb_ctx* ctx, const float* xt, const float* tvec, bool bi
   const int R = ctx->node_only ? V : E;
   const int rps = R / ctx->gn_segments;
   const int bps = (rps + GN_ROWS_PER_BLOCK - 1) / GN_ROWS_PER_BLOCK;
-  if (gn_fused_blocks > 0) {   // partial sums came out of the last edge layer's epilogue: no extra read of e
-    k_gn_final<<<dim3(1, 32), 256, 0, st>>>((const double*)ctx->gn_part.p, gn_fused_blocks, rps, (float*)ctx->gn_stats.p);
-    CKL(ctx);
-  } else {
-    k_gn_partial<<<dim3(bps, ctx->gn_segments), 256, 0, st>>>(Z, rps, (double*)ctx->gn_part.p);
-    CKL(ctx);
-    k_gn_final<<<dim3(ctx->gn_segments, 32), 256, 0, st>>>((const double*)ctx->gn_part.p, bps, rps, (float*)ctx->gn_stats.p);
-    CKL(ctx);
-  }
+  k_gn_partial<<<dim3(bps, ctx->gn_segments), 256, 0, st>>>(Z, rps, (double*)ctx->gn_part.p);
+  CKL(ctx);
+  k_gn_final<<<dim3(ctx->gn_segments, 32), 256, 0, st>>>((const double*)ctx->gn_part.p, bps, rps, (float*)ctx->gn_stats.p);
+  CKL(ctx);
   k_head<<<(R + 255) / 256, 256, 0, st>>>(Z, R, rps, (const float*)ctx->gn_stats.p, ctx->node_only ? nullptr : g.perm,
                                       ctx->hp, pa);
   CKL(ctx);
@@ -945,7 +893,7 @@ extern "C" int dfb_denoise(dfb_ctx* ctx, int diffusion_type, float* xt, int step
   if (want_graph) {
     dfb_ctx::LoopKey key;
     key.buf_gen = ctx->buf_gen; key.steps = steps; key.diffusion = diffusion_type; key.impl = ctx->edge_impl;
-    key.agg = ctx->agg_mode; key.pair = ctx->pair_enabled; key.uniforms = uniforms;
+    key.agg = ctx->agg_mode; key.uniforms = uniforms;
     if (!ctx->loop_exec || !(ctx->loop_key == key)) {
       if (ctx->loop_exec) {
         cudaGraphExecDestroy(ctx->loop_exec);
@@ -1044,8 +992,8 @@ extern "C" int dfb_profile_end(dfb_ctx* ctx, double* ms, int64_t* n) {
 
 // ================================================================================================
 // Test hook: run only GEMM1 of layer `layer` (acc = e_in * C^T, split-bf16 on tensor cores) on the
-// prepared graph's tiling and dump the TMEM accumulator.  Isolates descriptors / TMA / TMEM
-// plumbing from the epilogue math in tests/test_tc_gemm.py.
+// prepared graph's tiling and dump the accumulator.  Isolates descriptors / TMA / wgmma plumbing from the
+// epilogue math (tests/test_gpu_parity.py).
 extern "C" int dfb_debug_edge_gemm(dfb_ctx* ctx, int layer, const float* e_in, float* acc_out, void* stream_) {
   if (!ctx) return DFB_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream_;
@@ -1053,22 +1001,17 @@ extern "C" int dfb_debug_edge_gemm(dfb_ctx* ctx, int layer, const float* e_in, f
   if (!ctx->graph_ready) FAIL(ctx, DFB_E_INVALID, "dfb_prepare_graph must be called first");
   if (layer < 0 || layer >= ctx->L) FAIL(ctx, DFB_E_INVALID, "layer out of range");
   ctx->tc.debug_acc = acc_out;
-  int r;
-  if (ctx->edge_impl == DFB_EDGE_IMPL_TC && ctx->pair_enabled && ctx->max_seg <= v2::MAXSEG)
-    r = v2::launch(&ctx->pair, &ctx->tc, layer, const_cast<float*>(e_in), (const float*)ctx->uvab.p,
-                   (float*)ctx->partials.p, ctx->g, ctx->layers[layer], nullptr, AGG_SUM, st);
-  else
-    r = tc_launch_edge_layer(&ctx->tc, layer, const_cast<float*>(e_in), (const float*)ctx->uvab.p,
-                             (float*)ctx->partials.p, ctx->g, ctx->layers[layer], nullptr, 0, 0, nullptr,
-                             ctx->lut, AGG_SUM, st);
+  int r = tc_launch_edge_layer(&ctx->tc, layer, const_cast<float*>(e_in), (const float*)ctx->uvab.p,
+                               (float*)ctx->partials.p, ctx->g, ctx->layers[layer], nullptr, 0, 0, nullptr,
+                               ctx->lut, AGG_SUM, st, ctx->edge_impl == DFB_EDGE_IMPL_TC1 ? 1 : 2);
   ctx->tc.debug_acc = nullptr;
-  if (r) FAIL(ctx, DFB_E_CUDA, "tcgen05 edge layer: %s", ctx->tc.err.c_str());
+  if (r) FAIL(ctx, DFB_E_CUDA, "tensor-core edge layer: %s", ctx->tc.err.c_str());
   ctx->launches += 1;
   return DFB_OK;
 }
 
-// Test/tuning hook: read and reset the per-phase cycle counters of the tcgen05 edge kernel
-// (filled only when DFB_TC_PROBE has bit 7 set, --prof build).  out[32] host.
+// Test/tuning hook: read and reset the per-phase cycle counters of the edge kernel.  The wgmma kernels record
+// none, so the counters read back as zero.  out[32] host.
 extern "C" int dfb_debug_phase_cycles(dfb_ctx* ctx, unsigned long long* out) {
   if (!ctx || !out) return DFB_E_INVALID;
   CK(ctx, cudaSetDevice(ctx->device));
@@ -1078,17 +1021,7 @@ extern "C" int dfb_debug_phase_cycles(dfb_ctx* ctx, unsigned long long* out) {
   return DFB_OK;
 }
 
-#ifdef DFB_PHASE_PROF
-// Tuning build only (not part of the ABI): time line of cluster 0's leader CTA, see g_pair_trace in edge_layer_v2.cuh.  out[512].
-extern "C" int dfb_debug_pair_trace(long long* out) {
-  if (!out) return DFB_E_INVALID;
-  if (cudaDeviceSynchronize() != cudaSuccess) return DFB_E_CUDA;
-  if (cudaMemcpyFromSymbol(out, dfb::v2::g_pair_trace, sizeof(long long) * 512) != cudaSuccess) return DFB_E_CUDA;
-  return DFB_OK;
-}
-#endif
-
-// Diagnostic: watchdog record of the tcgen05 kernel (host-mapped, readable even after a launch failure):
+// Diagnostic: watchdog record of the tensor-core kernel (host-mapped, readable even after a launch failure):
 // out[0] = wait-site code (0 = none), out[1] = blockIdx.x, out[2] = parity waited for, out[3] = threadIdx.x.
 extern "C" int dfb_debug_watchdog(dfb_ctx* ctx, int* out) {
   if (!ctx || !out || !ctx->tc.error_host) return DFB_E_INVALID;

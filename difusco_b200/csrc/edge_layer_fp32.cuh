@@ -1,5 +1,5 @@
 // fp32 (FFMA) fused edge layer: the VALIDATION implementation of the hot kernel.
-// Same inputs, outputs, buffers and summation structure as the tcgen05 kernel in
+// Same inputs, outputs, buffers and summation structure as the wgmma kernel in
 // edge_layer_tc.cuh, but plain fp32 arithmetic, so tests can separate "algorithm wrong" from
 // "split-precision tensor-core path wrong".  Selected only through dfb_set_edge_impl (tests).
 //

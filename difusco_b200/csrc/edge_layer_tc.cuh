@@ -1,25 +1,24 @@
-// The hot kernel: one fused GNN edge layer on 5th-gen tensor cores (tcgen05 + TMEM + TMA), sm_100a.
+// The hot kernel: one fused GNN edge layer on Hopper tensor cores (wgmma + TMA + mbarrier), sm_90a.
 //
 //   e_hat = C e + A h[col] + B h[row]                         gnn_encoder.py:104,110
 //   agg  += sigmoid(e_hat) * V h[col]   (row-segment sums)     :112,163,177-191
 //   e_til = relu(LN_e(e_hat)) + tau                            :131,135,445
 //   e     = e + O silu(LN_O(e_til)) + b_O   (in place)         :449, :339-347
 //
-// Persistent CTAs, one per SM, each looping over 128-edge tiles (edges are row-sorted).
-// Warp roles (64 + 128*WPQ threads, WPQ = worker warps per TMEM lane quarter, default 4):
-//   warp 0       TMA producer: streams the bf16 hi/lo weight K-chunks (L2 -> smem, 128B swizzle), L2-prefetches the
-//                next tile's edge rows
-//   warp 1       MMA issuer  : one thread issues tcgen05.mma (M=128, N=256, K=16), owns the TMEM allocation.
-//                GEMM1 takes A from shared memory, GEMM2 takes A from TMEM (written in place by E3)
-//   worker warps thread == edge row == TMEM lane; the 256 channels of a row are split over the WPQ warps of a lane
-//                quarter.  They convert the fp32 edge tile to bf16 hi/lo A chunks and run the epilogues straight out
-//                of TMEM (a row slice lives in one thread: both LayerNorms are thread-local + one smem exchange).
-// Data movement: weights by TMA; gathers of A h[col], V h[col] by coalesced cp.async into swizzled staging; the
-// residual tile in and the result tile out by TMA (no uncoalesced global access on the edge stream).
+// Persistent CTAs, one per SM, each looping over tiles of 64 * NWG row-sorted edges.
+//   warps 0 .. 4 NWG - 1  NWG consumer warpgroups.  Warpgroup w owns rows [64 w, 64 w + 64) of a tile and keeps their
+//                         64 x 256 fp32 accumulator in registers (wgmma m64n256k16, A and B from shared memory).  It
+//                         converts its fp32 rows into the bf16 hi/lo A operand, runs GEMM1, the gate / message /
+//                         LayerNorm epilogues straight out of the accumulator registers (a row lives in the 4 threads
+//                         of a quad), writes GEMM2's A operand over GEMM1's and finishes with the residual update.
+//   warpgroup NWG         TMA producer (one thread): streams the bf16 hi/lo weight K-chunks [256 rows x 64 K] (128B
+//                         swizzle) through an NSTAGE ring that every consumer warpgroup reads.  With two consumer
+//                         warpgroups it hands its registers to them (setmaxnreg 40 / 232): no spills in the epilogue.
+// Per-(32-edge group, node) message sums go through shared memory (the dead GEMM1 operand) and are reduced in a fixed
+// order per column: deterministic, no atomics.
 // Precision: every 256x256 product is evaluated as  a_hi*b_hi + a_lo*b_hi + a_hi*b_lo  with
-// a = a_hi + a_lo, b = b_hi + b_lo in bf16 and fp32 accumulation in TMEM: ~2^-17 relative error
-// per product, which keeps the 1e-4 fp32 contract (single-pass TF32/BF16 does not: SURVEY D9).
-// The two 128x256 fp32 accumulators (GEMM1, GEMM2) take the full 512 TMEM columns.
+// a = a_hi + a_lo, b = b_hi + b_lo in bf16 and fp32 accumulation: ~2^-17 relative error per product, which keeps the
+// 1e-4 fp32 contract (single-pass TF32/BF16 does not: SURVEY D9).
 // The same kernel in "linear mode" computes the node-side linears and the embedding linears (GEMM1 + bias only).
 #pragma once
 #include <cuda.h>
@@ -35,18 +34,27 @@
 
 namespace dfb {
 
-constexpr int TC_TILE = 128;
-constexpr int TC_KCH = 64;                         // K elements per chunk = one 128-byte swizzle row
-constexpr int TC_A_BYTES = TC_TILE * 128;          // 16 KB  (hi or lo)
-constexpr int TC_B_BYTES = 256 * 128;              // 32 KB  (hi or lo)
-constexpr int TC_STAGE_BYTES = 2 * TC_A_BYTES + 2 * TC_B_BYTES;   // 96 KB per stage, laid out A0 | A1 | B0 | B1
-__host__ __device__ constexpr int tc_off_a(int s) { return s * 2 * TC_A_BYTES; }
-__host__ __device__ constexpr int tc_off_b(int s) { return 4 * TC_A_BYTES + s * 2 * TC_B_BYTES; }
-constexpr int TC_BOX_BYTES = TC_TILE * 128;        // one fp32 [128 rows x 32 cols] TMA box of the edge stream
-constexpr int TC_NSTAGE = 2;
-constexpr int TC_OFF_PRM = TC_NSTAGE * TC_STAGE_BYTES;            // 6 x 256 floats
-// UMMA instruction descriptor: D=F32, A=B=BF16, both K-major, N=256, M=128 (cute::UMMA::InstrDescriptor)
-constexpr uint32_t TC_IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((256u >> 3) << 17) | ((128u >> 4) << 24);
+constexpr int WG_ROWS = 64;                     // rows per consumer warpgroup (wgmma M)
+constexpr int TC_KCH = 64;                      // K elements per chunk = one 128-byte swizzle row of bf16
+constexpr int TC_B_BYTES = 256 * 128;           // one weight chunk [256 rows x 64 K] bf16 (hi or lo)
+constexpr int TC_A_CHUNK = WG_ROWS * 128;       // one operand chunk [64 rows x 64 K] bf16 (hi or lo)
+constexpr int TC_A_BYTES = 8 * TC_A_CHUNK;      // 4 K-chunks x (hi, lo) per warpgroup = 64 KB = [64][256] fp32 messages
+
+template <int NWG>
+struct TcCfg {
+  static_assert(NWG == 1 || NWG == 2, "one or two consumer warpgroups");
+  static constexpr int TILE = NWG * WG_ROWS;
+  static constexpr int THREADS = (NWG + 1) * 128;
+  static constexpr int NSTAGE = (NWG == 1) ? 3 : 2;
+  static constexpr int OFF_B = NWG * TC_A_BYTES;
+  static constexpr int OFF_PRM = OFF_B + NSTAGE * TC_B_BYTES;   // ln_e_g, ln_e_b, tau, ln_o_g, ln_o_b, b_O
+  static constexpr int OFF_ROW = OFF_PRM + 6 * H * 4;
+  static constexpr int OFF_SRC = OFF_ROW + TILE * 4;
+  static constexpr int OFF_BAR = OFF_SRC + TILE * 8;
+  static constexpr int SMEM_BYTES = OFF_BAR + 2 * NSTAGE * 8;
+  static constexpr int SMEM_ALLOC = SMEM_BYTES + 1024;          // slack for 1024-byte alignment
+  static_assert(SMEM_ALLOC <= 232448, "shared memory budget (227 KB per block)");
+};
 
 struct TcParams {
   float* e;
@@ -59,8 +67,8 @@ struct TcParams {
   const float* lut;       // [2][256]
   const float* zero_row;  // [256] zeros
   float* debug_acc;       // tests: dump GEMM1 accumulator [E][256] and stop
-  // linear mode (node-side linears on the same tensor-core path): rows of lin_in [lin_rows][256] times the four
-  // 256x256 blocks U|V|A|B -> lin_out [lin_rows][1024] (+ lin_bias[1024]).  tile = row_tile * 4 + block.
+  // linear mode: rows of lin_in [lin_rows][256] times lin_nb 256x256 blocks -> lin_out [lin_rows][lin_nb * 256]
+  // (+ lin_bias).  tile = row_tile * lin_nb + block.
   const float* lin_in;
   float* lin_out;
   const float* lin_bias;
@@ -71,9 +79,6 @@ struct TcParams {
   int write_e, e_zero, agg_mode;
   int w_row_base;         // row of this layer's C_hi block in the bf16 weight arena tensor map
   int n_tiles;
-  unsigned long long* phase_cycles;   // [16] probe bit 7: per-phase cycle sums of worker thread 0, all CTAs
-  int probe;   // timing experiments only (DFB_TC_PROBE env): bit 0 = E1 without its gather data (--prof tuning build only),
-               // bit 7 = per-phase cycle counters (--prof build), bit 8 = no L2 prefetch of the next tile
 };
 
 // ----------------------------------------------------------------------------------------------
@@ -90,9 +95,6 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-#ifndef DFB_WAIT_HINT_NS
-#define DFB_WAIT_HINT_NS 20000u
-#endif
 // Bounded wait: a protocol bug must surface as a launch failure, not as a hung GPU.  try_wait suspends
 // the thread in hardware (up to the hint, in ns) instead of burning issue slots.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int* error_flag, int code) {
@@ -103,7 +105,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int* e
     asm volatile(
         "{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n selp.u32 %0, 1, 0, p;\n}"
         : "=r"(ok)
-        : "r"(addr), "r"(parity), "r"(DFB_WAIT_HINT_NS)
+        : "r"(addr), "r"(parity), "r"(20000u)
         : "memory");
     if (ok) return;
     if (spin > 400000u) {   // >> any legitimate wait (each failed try_wait already slept up to 20 us)
@@ -124,108 +126,52 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+// K-major, 128-byte swizzle, 8-row atoms 1024 bytes apart (wgmma shared-memory matrix descriptor)
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr >> 4) & 0x3fffu) | (1ull << 16) | (64ull << 32) | (1ull << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma window.
+__device__ __forceinline__ void acc_fence(float (&d)[128]) {
+#pragma unroll
+  for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// D[64 x 256] (+)= A[64 x 16] * B[256 x 16]^T, bf16 in, fp32 accumulate; scale_d == 0 overwrites D
+__device__ __forceinline__ void wgmma_bf16(float (&d)[128], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n"
-      " tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(TC_IDESC), "r"(accumulate)
-      : "memory");
-}
-// A operand from tensor memory (lane = row, 32-bit columns = packed bf16 pairs along K), B from shared memory
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n"
-      " tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(TC_IDESC), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// K-major, 128-byte swizzle, 8-row atoms 1024 bytes apart (cute::UMMA::SmemDescriptor, version 1)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  const uint64_t hi = 64ull | (1ull << 14) | (2ull << 29);
-  return (hi << 32) | (1ull << 16) | (uint64_t)((smem_addr >> 4) & 0x3fffu);
-}
-
-#define TC_R32(v) \
-  "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),       \
-  "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),            \
-  "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),           \
-  "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-#define TC_W32(v) \
-  "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),     \
-  "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),       \
-  "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),       \
-  "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-
-// 32 lanes x 32 columns: thread <lane> of the warp gets 32 consecutive fp32 columns of its TMEM lane
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      "{\n .reg .pred p;\n setp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : TC_R32(v)
-      : "r"(taddr)
-      : "memory");
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%32], "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31};"
-      ::TC_W32(v), "r"(taddr)
-      : "memory");
-}
-#define TC_R16(v) \
-  "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),       \
-  "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-#define TC_W16(v) \
-  "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),     \
-  "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : TC_R16(v)
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%16], "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15};"
-      ::TC_W16(v), "r"(taddr)
-      : "memory");
-}
-// Ampere-style 16-byte async copy global -> shared (LDGSTS): coalesced gathers without register staging
-__device__ __forceinline__ void cp_async16(uint32_t dst_smem, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst_smem), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-// TMA store smem -> global (bulk async-group completion)
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-template <int N> __device__ __forceinline__ void tmem_ldN(uint32_t taddr, uint32_t (&v)[N]);
-template <> __device__ __forceinline__ void tmem_ldN<16>(uint32_t taddr, uint32_t (&v)[16]) { tmem_ld16(taddr, v); }
-template <> __device__ __forceinline__ void tmem_ldN<32>(uint32_t taddr, uint32_t (&v)[32]) { tmem_ld32(taddr, v); }
-template <int N> __device__ __forceinline__ void tmem_stN(uint32_t taddr, const uint32_t (&v)[N]);
-template <> __device__ __forceinline__ void tmem_stN<16>(uint32_t taddr, const uint32_t (&v)[16]) { tmem_st16(taddr, v); }
-template <> __device__ __forceinline__ void tmem_stN<32>(uint32_t taddr, const uint32_t (&v)[32]) { tmem_st32(taddr, v); }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // sigmoid with one MUFU.EX2 and one MUFU.RCP (ex2.approx: 2 ulp, rcp.approx: 1 ulp -> ~3e-7 relative)
 __device__ __forceinline__ float sigmoid_mufu(float x) {
@@ -233,37 +179,6 @@ __device__ __forceinline__ float sigmoid_mufu(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(-1.4426950408889634f * x));
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + t));
   return r;
-}
-// Packed fp32x2 arithmetic (Blackwell FADD2 / FMUL2 / FFMA2): two independent IEEE fp32 operations per instruction
-__device__ __forceinline__ float2 add2(float2 a, float2 b) {
-  float2 d;
-  asm("{.reg .b64 ra, rb, rd; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%5}; add.rn.f32x2 rd, ra, rb; mov.b64 {%0,%1}, rd;}"
-      : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return d;
-}
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-  float2 d;
-  asm("{.reg .b64 ra, rb, rd; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%5}; mul.rn.f32x2 rd, ra, rb; mov.b64 {%0,%1}, rd;}"
-      : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return d;
-}
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-  float2 d;
-  asm("{.reg .b64 ra, rb, rc, rd; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%5}; mov.b64 rc, {%6,%7}; "
-      "fma.rn.f32x2 rd, ra, rb, rc; mov.b64 {%0,%1}, rd;}"
-      : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-  return d;
-}
-__device__ __forceinline__ float2 splat2(float a) { return make_float2(a, a); }
-__device__ __forceinline__ float2 sigmoid_mufu2(float2 x) {
-  const float2 t = mul2(x, splat2(-1.4426950408889634f));
-  float e0, e1, r0, r1;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(t.x));
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(t.y));
-  const float2 y = add2(make_float2(e0, e1), splat2(1.0f));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r0) : "f"(y.x));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r1) : "f"(y.y));
-  return make_float2(r0, r1);
 }
 // fp32 x4 -> bf16 hi x4, bf16 lo x4 (lo = rn(x - hi))
 __device__ __forceinline__ void split4(float4 x, uint2& hi, uint2& lo) {
@@ -276,80 +191,51 @@ __device__ __forceinline__ void split4(float4 x, uint2& hi, uint2& lo) {
   lo.x = *reinterpret_cast<uint32_t*>(&l01);
   lo.y = *reinterpret_cast<uint32_t*>(&l23);
 }
+__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
+  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  const float2 f = __bfloat1622float2(h);
+  __nv_bfloat162 l = __floats2bfloat162_rn(a - f.x, b - f.y);
+  hi = *reinterpret_cast<uint32_t*>(&h);
+  lo = *reinterpret_cast<uint32_t*>(&l);
+}
 // byte offset of (row r, 16-byte unit j in [0,8)) inside a [rows][64 bf16] K-major 128B-swizzled tile
 __device__ __forceinline__ uint32_t sw128_off(int r, int j) {
   return (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((j ^ (r & 7)) << 4));
 }
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
 
 // ----------------------------------------------------------------------------------------------
-// WPQ = worker warps per TMEM lane quarter.  The 256 channels of a row are split into WPQ contiguous
-// slices, one per warp of the quarter (warps with equal warp_id % 4 may touch the same TMEM lanes);
-// LayerNorm partial statistics of the slices are combined through shared memory.
-template <int WPQ>
-struct TcCfg {
-  static_assert(WPQ == 1 || WPQ == 2 || WPQ == 4, "1, 2 or 4 worker warps per TMEM lane quarter");
-  static constexpr int NWORK = 128 * WPQ;                 // worker threads
-  static constexpr int THREADS = 64 + NWORK;
-  static constexpr int CPP = H / WPQ;                     // columns per part
-  static constexpr int PATCH_COLS = (WPQ == 4) ? 8 : 16;  // columns per segment-reduce pass (E1 sub-chunk = 16 columns)
-  static constexpr int CW = (WPQ == 4) ? 16 : 32;         // TMEM chunk width of E2/E3/E4 (register budget)
-  static_assert((TC_KCH / WPQ) % CW == 0, "a part's slice of a K-chunk must be whole TMEM chunks");
-  static constexpr bool PREFETCH = (WPQ != 4);            // register prefetch of the next sub-chunk (register budget)
-  static constexpr bool GATE_B0 = (WPQ == 4);             // gather buffers spill into B0: GEMM2's first weights wait for E1
-  static constexpr int OFF_PATCH = TC_OFF_PRM + 6 * H * 4;   // per warp PATCH_COLS x 36 floats; also carries the LN statistics
-  static constexpr int OFF_ROW = OFF_PATCH + 4 * WPQ * PATCH_COLS * 36 * 4;
-  static constexpr int OFF_COL = OFF_ROW + TC_TILE * 4;
-  static constexpr int OFF_SRC = OFF_COL + TC_TILE * 4;
-  static constexpr int OFF_BAR = OFF_SRC + TC_TILE * 8;
-  static constexpr int SMEM_BYTES = OFF_BAR + 128;
-  static constexpr int SMEM_ALLOC = SMEM_BYTES + 1024;    // slack for 1024-byte alignment
-  static_assert(SMEM_ALLOC <= 232448, "shared memory budget");
-  static_assert(PATCH_COLS * 36 >= 192, "patch must hold the per-warp LayerNorm statistics");
-};
-
-template <int WPQ>
-__device__ __forceinline__ void edge_layer_tc_body(const CUtensorMap& wmap, const CUtensorMap& emap, const TcParams& P) {
-  using Cfg = TcCfg<WPQ>;
+// Accumulator fragment of wgmma m64n256 (per thread: warp wi of the warpgroup, lane = 4 * g + t):
+//   acc[4 j + 2 h + b]  ->  row 16 wi + g + 8 h,  column 8 j + 2 t + b        (j < 32, h, b in {0, 1})
+// so the 256 columns of a row are spread over the 4 threads of a quad: row reductions are 64 thread-local terms
+// plus two shuffles.
+// ----------------------------------------------------------------------------------------------
+template <int NWG>
+__device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, const TcParams& P) {
+  using Cfg = TcCfg<NWG>;
+  constexpr int NSTAGE = Cfg::NSTAGE;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // stays in .shared
-  float* prm = reinterpret_cast<float*>(smem + TC_OFF_PRM);      // ln_e_g, ln_e_b, tau, ln_o_g, ln_o_b, b_O
-  float* patch_all = reinterpret_cast<float*>(smem + Cfg::OFF_PATCH);
+  float* prm = reinterpret_cast<float*>(smem + Cfg::OFF_PRM);
   int* s_row = reinterpret_cast<int*>(smem + Cfg::OFF_ROW);
-  int* s_col = reinterpret_cast<int*>(smem + Cfg::OFF_COL);
   const float** s_src = reinterpret_cast<const float**>(smem + Cfg::OFF_SRC);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
-  uint64_t* full_a1 = bars;       // [2] all workers -> MMA (GEMM1 A chunks in smem stage s, NWORK arrivals)
-  uint64_t* full_a2 = bars + 2;   // [4] all workers -> MMA (GEMM2 A chunk kc written to TMEM).  One barrier PER CHUNK,
-                                  //     completing once per tile: E3 has no back-pressure from the MMA any more (the A
-                                  //     operand lives in TMEM, no stage to wait for), so two chunks must never share a
-                                  //     barrier - the workers could run two phases ahead of the MMA thread's parity wait.
-  uint64_t* full_b = bars + 6;    // [2] TMA -> MMA (expect_tx)
-  uint64_t* empty = bars + 8;     // [2] MMA commit -> producer + workers
-  uint64_t* acc_rdy = bars + 10;  // [2] MMA commit -> workers (GEMM1 / GEMM2 accumulator complete)
-  uint64_t* ein_bar = bars + 12;  // TMA load of the residual tile (expect_tx)
-  uint64_t* e4_done = bars + 13;  // staging (A0|A1|B0) released after the TMA store has read it
-  uint64_t* e1_done = bars + 14;  // all warps left E1: the B0 region no longer holds gather buffers (GATE_B0)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 15);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);   // [NSTAGE] TMA -> consumers (expect_tx)
+  uint64_t* empty = full + NSTAGE;                                      // [NSTAGE] every consumer warp -> producer
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int uses_per_tile = P.write_e ? 8 : 4;
+  const bool lin = P.lin_out != nullptr;
+  const int loads_per_tile = P.write_e ? 16 : 8;   // (C | O) x 4 K-chunks x (hi, lo)
 
   if (threadIdx.x == 0) {
-    mbar_init(&full_a1[0], Cfg::NWORK); mbar_init(&full_a1[1], Cfg::NWORK);
-    mbar_init(&full_a2[0], Cfg::NWORK); mbar_init(&full_a2[1], Cfg::NWORK);
-    mbar_init(&full_a2[2], Cfg::NWORK); mbar_init(&full_a2[3], Cfg::NWORK);
-    mbar_init(&full_b[0], 1);           mbar_init(&full_b[1], 1);
-    mbar_init(&empty[0], 1);            mbar_init(&empty[1], 1);
-    mbar_init(&acc_rdy[0], 1);          mbar_init(&acc_rdy[1], 1);
-    mbar_init(ein_bar, 1);              mbar_init(e4_done, 1);
-    mbar_init(e1_done, 1);
+    for (int s = 0; s < NSTAGE; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 4 * NWG);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     fence_proxy_async();
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   for (int i = threadIdx.x; i < H; i += Cfg::THREADS) {
     prm[i] = P.lp.ln_e_g[i];
@@ -359,626 +245,273 @@ __device__ __forceinline__ void edge_layer_tc_body(const CUtensorMap& wmap, cons
     prm[4 * H + i] = P.lp.ln_o_b[i];
     prm[5 * H + i] = P.lp.b_O[i];
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const uint32_t smem_base = smem_u32(smem);
 
-  if (warp == 0) {
+  if (warp >= 4 * NWG) {
     // ===================================== TMA producer =====================================
-    if (lane == 0) {
-      uint32_t u = 0, tile_it = 0;
-      const bool tma_in = !P.e_zero && !P.xt_lut;   // residual tile comes from the edge stream (not LUT / zero rows)
-      for (int tile = blockIdx.x; tile < P.n_tiles; tile += gridDim.x, ++tile_it) {
-        // E4 of the previous tile stages its output in A0|A1|B0: do not refill B0 before the store has read it
-        if (P.write_e && tile_it > 0) mbar_wait(e4_done, (tile_it - 1) & 1, P.error_flag, 8);
-        if (!P.lin_out && !P.e_zero && !P.xt_lut && tile + (int)gridDim.x < P.n_tiles && !(P.probe & 256)) {
-          // the next tile's 128 edge rows are one contiguous 128 KB block: pull it into L2 now
-          const float* nxt = P.e + (size_t)(tile + gridDim.x) * TC_TILE * H;
-          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(nxt), "r"(TC_TILE * H * 4) : "memory");
-        }
-        for (int i = 0; i < uses_per_tile; ++i, ++u) {
-          const int s = u & 1, k = u >> 1, kc = i & 3;
-          mbar_wait(&empty[s], (k & 1) ^ 1, P.error_flag, 1);
-          if (i == 4) {
-            // every warp has left E1: the A-stage memory (gather buffers) is idle for the rest of the tile (GEMM2 takes
-            // its A operand from TMEM) -> bring in boxes 0..3 of the fp32 residual tile for E4 now; with GATE_B0 this
-            // also releases B0 for GEMM2's first weights
-            mbar_wait(e1_done, tile_it & 1, P.error_flag, 11);
-            if (tma_in) {
-              mbar_arrive_expect_tx(ein_bar, 8 * TC_BOX_BYTES);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) tma_load_2d(smem_base + j * TC_BOX_BYTES, &emap, ein_bar, 32 * j, tile * TC_TILE);
-            }
-          }
-          // without GEMM2 (MIS last layer) the next fill of B0 is the NEXT tile's first chunk: same gate, previous tile
-          if (Cfg::GATE_B0 && i == 0 && tile_it > 0 && !P.write_e && !P.lin_out && !P.debug_acc)
-            mbar_wait(e1_done, (tile_it - 1) & 1, P.error_flag, 12);
-          mbar_arrive_expect_tx(&full_b[s], 2 * TC_B_BYTES);
-          const uint32_t dst = smem_base + tc_off_b(s);
-          // C_hi,C_lo | O_hi,O_lo blocks of 256 rows; linear mode: U|V|A|B (hi,lo) blocks follow at +1024
-          const int rb = P.lin_out ? P.lin_w_row + (P.lin_nb == 4 ? (tile & 3) : 0) * 512 : P.w_row_base + (i < 4 ? 0 : 512);
-          const int kw = kc;
-          tma_load_2d(dst, &wmap, &full_b[s], kw * TC_KCH, rb);
-          tma_load_2d(dst + TC_B_BYTES, &wmap, &full_b[s], kw * TC_KCH, rb + 256);
-        }
-        if (P.write_e && tma_in) {
-          // boxes 4..7 of the residual tile land in B0: free once GEMM2's stage-0 MMAs (use 6 of this tile) are done
-          mbar_wait(&empty[0], ((u - 2) >> 1) & 1, P.error_flag, 14);
-#pragma unroll
-          for (int j = 4; j < 8; ++j) tma_load_2d(smem_base + j * TC_BOX_BYTES, &emap, ein_bar, 32 * j, tile * TC_TILE);
+    if constexpr (NWG == 2) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == 4 * NWG && lane == 0) {
+      uint32_t u = 0;
+      for (int tile = blockIdx.x; tile < P.n_tiles; tile += gridDim.x) {
+        for (int i = 0; i < loads_per_tile; ++i, ++u) {
+          const int s = u % NSTAGE;
+          mbar_wait(&empty[s], ((u / NSTAGE) & 1) ^ 1, P.error_flag, 1);
+          mbar_arrive_expect_tx(&full[s], TC_B_BYTES);
+          // C_hi,C_lo | O_hi,O_lo blocks of 256 rows; linear mode: U|V|A|B (hi,lo) blocks 512 rows apart
+          const int row = (lin ? P.lin_w_row + (P.lin_nb == 4 ? (tile & 3) : 0) * 512 : P.w_row_base + (i >= 8 ? 512 : 0)) +
+                          (i & 1) * 256;
+          tma_load_2d(smem_base + Cfg::OFF_B + s * TC_B_BYTES, &wmap, &full[s], ((i >> 1) & 3) * TC_KCH, row);
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================================== MMA issuer =======================================
-    if (lane == 0) {
-      uint32_t u = 0, tile_it = 0;
-      for (int tile = blockIdx.x; tile < P.n_tiles; tile += gridDim.x, ++tile_it) {
-        for (int i = 0; i < uses_per_tile; ++i, ++u) {
-          const int s = u & 1, k = u >> 1, kc = i & 3;
-          mbar_wait(&full_b[s], k & 1, P.error_flag, 2);
-          // full_a1[s] completes twice per tile (chunks kc, kc+2; conv waits for empty[s] in between): parity (kc>>1)&1.
-          // full_a2[kc] completes once per tile: parity tile_it & 1.
-          if (i < 4) mbar_wait(&full_a1[s], (kc >> 1) & 1, P.error_flag, 3);
-          else mbar_wait(&full_a2[kc], tile_it & 1, P.error_flag, 13);
-          tc_fence_after();
-          const uint32_t a_hi = smem_base + tc_off_a(s), a_lo = a_hi + TC_A_BYTES;
-          const uint32_t b_hi = smem_base + tc_off_b(s), b_lo = b_hi + TC_B_BYTES;
-          const uint32_t d = tmem_base + (i < 4 ? 0u : 256u);
-          if (i < 4) {
+    return;
+  }
+
+  // ===================================== consumer warpgroups =====================================
+  if constexpr (NWG == 2) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  const int wg = warp >> 2, wi = warp & 3, tid = threadIdx.x & 127;
+  const int t4 = lane & 3;
+  const int lr0 = wi * 16 + (lane >> 2);   // this thread's rows inside the warpgroup: lr0, lr0 + 8
+  unsigned char* a_reg = smem + wg * TC_A_BYTES;
+  const uint32_t a_base = smem_base + wg * TC_A_BYTES;
+  float* msg = reinterpret_cast<float*>(a_reg);   // [64][256] fp32, column c of row r at c ^ 8 (r & 7)
+  int* w_row = s_row + wg * WG_ROWS;
+  const float** w_src = s_src + wg * WG_ROWS;
+  auto wg_bar = [&] { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); };
+  const int n_rows = lin ? P.lin_rows : P.g.E;
+  uint32_t u = 0;
+  float acc[128];
+
+  // 8 weight chunks (4 K-chunks x hi, lo) against this warpgroup's A operand (hi, lo at chunk 2 kc, 2 kc + 1)
+  auto gemm = [&]() {
+    acc_fence(acc);
+    wgmma_fence();
 #pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-              const uint64_t dah = umma_desc_sw128(a_hi + ks * 32), dal = umma_desc_sw128(a_lo + ks * 32);
-              const uint64_t dbh = umma_desc_sw128(b_hi + ks * 32), dbl = umma_desc_sw128(b_lo + ks * 32);
-              umma_bf16(d, dah, dbh, (kc | ks) ? 1u : 0u);
-              umma_bf16(d, dal, dbh, 1u);
-              umma_bf16(d, dah, dbl, 1u);
-            }
-          } else {
-            // GEMM2: the A operand (bf16 hi/lo of s) was written by E3 IN PLACE over e_til in the GEMM1 accumulator
-            // columns: k-step ks of chunk kc sits at columns 64 kc + 16 ks (8 columns hi, 8 columns lo)
+    for (int i = 0; i < 8; ++i, ++u) {
+      const int s = u % NSTAGE;
+      mbar_wait(&full[s], (u / NSTAGE) & 1, P.error_flag, 2);
+      const uint32_t b = smem_base + Cfg::OFF_B + s * TC_B_BYTES;
+      const uint32_t ahi = a_base + (i >> 1) * 2 * TC_A_CHUNK, alo = ahi + TC_A_CHUNK;
 #pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-              const uint32_t ta_hi = tmem_base + kc * 64 + ks * 16, ta_lo = ta_hi + 8;
-              const uint64_t dbh = umma_desc_sw128(b_hi + ks * 32), dbl = umma_desc_sw128(b_lo + ks * 32);
-              umma_bf16_ts(d, ta_hi, dbh, (kc | ks) ? 1u : 0u);
-              umma_bf16_ts(d, ta_lo, dbh, 1u);
-              umma_bf16_ts(d, ta_hi, dbl, 1u);
-            }
-          }
-          umma_commit(&empty[s]);                       // frees the stage when these MMAs have read it
-          if (kc == 3) umma_commit(&acc_rdy[i < 4 ? 0 : 1]);
-        }
+      for (int ks = 0; ks < 4; ++ks) {
+        const uint64_t db = wgmma_desc_sw128(b + ks * 32);
+        wgmma_bf16(acc, wgmma_desc_sw128(ahi + ks * 32), db, (i | ks) ? 1u : 0u);   // hi*hi (B hi) or hi*lo (B lo)
+        if ((i & 1) == 0) wgmma_bf16(acc, wgmma_desc_sw128(alo + ks * 32), db, 1u);   // lo*hi
       }
+      wgmma_commit();
+      wgmma_wait_all();
+      acc_fence(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s]);
     }
-  } else {
-    // ===================================== row workers ======================================
-    const int q = warp & 3;                 // TMEM lane quarter this warp may access (hardware rule)
-    const int part = (warp - 2) >> 2;       // which column slice of the row
-    const int r = q * 32 + lane;            // tile row == TMEM lane
-    const int wt = (warp - 2) * 32 + lane;  // worker thread index, 0 .. NWORK-1
-    const int cbase = part * Cfg::CPP;
-    float* patch = patch_all + (warp - 2) * Cfg::PATCH_COLS * 36;
-    const uint32_t t_acc1 = tmem_base + ((uint32_t)(q * 32) << 16);
-    const uint32_t t_acc2 = t_acc1 + 256u;
-    auto worker_bar = [] { asm volatile("bar.sync 1, %0;" ::"n"(Cfg::NWORK) : "memory"); };
-#ifdef DFB_PHASE_PROF   // tuning build only (python -m difusco_b200.build --prof): per-phase clock64 counters of worker thread 0
-    const bool prof = (P.probe & 128) && wt == 0;
-    long long pc[16] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0}, tp = 0, tq = 0;
-#define PHASE(i) do { if (prof) { long long _n = clock64(); pc[i] += _n - tp; tp = _n; } } while (0)
-#define SUBPH(i) do { if (prof) { long long _n = clock64(); pc[i] += _n - tq; tq = _n; } } while (0)
-#define PROF_TILE_START() do { if (prof) tp = clock64(); } while (0)
-#define PROF_SUB_START() do { if (prof) tq = clock64(); } while (0)
-#else
-#define PHASE(i) do { } while (0)
-#define SUBPH(i) do { } while (0)
-#define PROF_TILE_START() do { } while (0)
-#define PROF_SUB_START() do { } while (0)
-#endif
-    uint32_t u_tile = 0;
-    for (int tile = blockIdx.x; tile < P.n_tiles; tile += gridDim.x, u_tile += uses_per_tile) {
-      PROF_TILE_START();
-      const int s_edge = ((P.lin_out && P.lin_nb == 4) ? (tile >> 2) : tile) * TC_TILE + r;
-      const bool valid = s_edge < (P.lin_out ? P.lin_rows : P.g.E);
-      int my_row = -1, my_col = 0;
+  };
+
+  for (int tile = blockIdx.x; tile < P.n_tiles; tile += gridDim.x) {
+    const int row_tile = (lin && P.lin_nb == 4) ? (tile >> 2) : tile;
+    const int s_base = row_tile * Cfg::TILE + wg * WG_ROWS;   // first edge (input row) of this warpgroup
+    if (tid < WG_ROWS) {
+      const int s = s_base + tid;
       const float* src = P.zero_row;
-      if (valid && P.lin_out) {
-        src = P.lin_in + (size_t)s_edge * H;
-      } else if (valid) {
-        my_row = P.g.row[s_edge];
-        my_col = P.g.col[s_edge];
+      int rw = -1;
+      if (s < n_rows && lin) {
+        src = P.lin_in + (size_t)s * H;
+      } else if (s < n_rows) {
+        rw = P.g.row[s];
         if (P.e_zero) src = P.zero_row;
-        else if (P.xt_lut) src = P.lut + ((P.xt_lut[P.g.perm ? P.g.perm[s_edge] : s_edge] != 0.0f) ? H : 0);
-        else src = P.e + (size_t)s_edge * H;
+        else if (P.xt_lut) src = P.lut + ((P.xt_lut[P.g.perm ? P.g.perm[s] : s] != 0.0f) ? H : 0);
+        else src = P.e + (size_t)s * H;
       }
-      if (part == 0) {
-        s_row[r] = my_row;
-        s_col[r] = my_col;
-        s_src[r] = src;
-      }
-      uint32_t seg_mask;
-      {
-        int next_row = __shfl_down_sync(0xffffffffu, my_row, 1);
-        bool seg_end = valid && (lane == 31 || next_row != my_row);
-        seg_mask = __ballot_sync(0xffffffffu, seg_end);
-      }
-      worker_bar();   // s_src / s_row of the whole tile visible to every worker
-
-      // ---------------- GEMM1 A operand: fp32 edge rows -> bf16 hi/lo swizzled chunks ----------------
-      constexpr int CONV_IT = 16 / WPQ;
-      float4 xa[CONV_IT], xb[CONV_IT];
-      auto conv_load = [&](float4 (&x)[CONV_IT], int kc) {
-#pragma unroll
-        for (int it = 0; it < CONV_IT; ++it) {
-          const int item = it * Cfg::NWORK + wt;
-          x[it] = __ldcg(reinterpret_cast<const float4*>(s_src[item >> 4] + kc * TC_KCH) + (item & 15));
-        }
-      };
-      auto conv_store = [&](const float4 (&x)[CONV_IT], int kc) {
-        const uint32_t u = u_tile + kc;
-        const int s = u & 1, k = u >> 1;
-        mbar_wait(&empty[s], (k & 1) ^ 1, P.error_flag, 4);
-        unsigned char* a_hi = smem + tc_off_a(s);
-        unsigned char* a_lo = a_hi + TC_A_BYTES;
-#pragma unroll
-        for (int it = 0; it < CONV_IT; ++it) {
-          const int item = it * Cfg::NWORK + wt;
-          const int rr = item >> 4, k4 = item & 15;
-          uint2 hi, lo;
-          split4(x[it], hi, lo);
-          const uint32_t off = sw128_off(rr, k4 >> 1) + (k4 & 1) * 8;
-          *reinterpret_cast<uint2*>(a_hi + off) = hi;
-          *reinterpret_cast<uint2*>(a_lo + off) = lo;
-        }
-        fence_proxy_async();
-        tc_fence_before();   // orders this thread's earlier TMEM reads (previous tile) before the MMA overwrites
-        mbar_arrive(&full_a1[s]);
-      };
-      conv_load(xa, 0);
-      conv_load(xb, 1);
-      // the previous tile's TMA store must have finished reading the staging area (A0|A1|B0)
-      if (P.write_e && u_tile > 0) mbar_wait(e4_done, ((u_tile / uses_per_tile) - 1) & 1, P.error_flag, 9);
-      conv_store(xa, 0);
-      conv_load(xa, 2);
-      conv_store(xb, 1);
-      conv_load(xb, 3);
-      conv_store(xa, 2);
-      conv_store(xb, 3);
-
-      PHASE(0);   // setup + conversion
-      // ---------------- E1: e_hat, gate, messages, row statistics ----------------
-      const uint32_t tile_par = (u_tile / uses_per_tile) & 1;
-      mbar_wait(&acc_rdy[0], tile_par, P.error_flag, 5);
-      tc_fence_after();
-      PHASE(1);   // wait for GEMM1
-      if (P.lin_out) {
-        const int nb = (P.lin_nb == 4) ? (tile & 3) : 0;
-        const int ostride = P.lin_nb * H;
-#pragma unroll 1
-        for (int c0 = cbase; c0 < cbase + Cfg::CPP; c0 += 32) {
-          uint32_t v[32];
-          tmem_ld32(t_acc1 + c0, v);
-          tmem_wait_ld();
-          if (valid) {
-            const float4* bias = reinterpret_cast<const float4*>(P.lin_bias + nb * H + c0);
-            float4* dst = reinterpret_cast<float4*>(P.lin_out + (size_t)s_edge * ostride + nb * H + c0);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float4 b4 = __ldg(bias + j);
-              __stcg(dst + j, make_float4(__uint_as_float(v[4 * j]) + b4.x, __uint_as_float(v[4 * j + 1]) + b4.y,
-                                          __uint_as_float(v[4 * j + 2]) + b4.z, __uint_as_float(v[4 * j + 3]) + b4.w));
-            }
-          }
-        }
-        tc_fence_before();
-        continue;
-      }
-      if (P.debug_acc) {
-#pragma unroll 1
-        for (int c0 = cbase; c0 < cbase + Cfg::CPP; c0 += 32) {
-          uint32_t v[32];
-          tmem_ld32(t_acc1 + c0, v);
-          tmem_wait_ld();
-          if (valid) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              __stcg(reinterpret_cast<float4*>(P.debug_acc + (size_t)s_edge * H + c0) + j,
-                     make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
-                                 __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3])));
-          }
-        }
-        tc_fence_before();
-        continue;
-      }
-      const float* uv_row = P.uvab + (size_t)(valid ? my_row : 0) * 4 * H;
-      const int grp = tile * 4 + q;
-      const int first_node = (grp < P.g.n_groups) ? P.g.grp_first[grp] : 0;
-      const size_t pair_base = (grp < P.g.n_groups) ? (size_t)P.g.grp_pair[grp] : 0;
-      // A h[col] and V h[col] are gathered with coalesced 16-byte cp.async (lanes along channels) into
-      // 128B-swizzled staging rows [A 16 cols | V 16 cols]; the stage-A operand memory is idle during E1.
-      // Every warp stages only its own 32 rows (two 4 KB buffers: sub-chunk i+1 in flight while i is consumed),
-      // so __syncwarp is the only synchronisation.  TMEM data and the B h[row] values of the next sub-chunk are
-      // prefetched into registers.
-      unsigned char* gbuf0 = smem + (warp - 2) * 8192;   // WPQ 1,2: inside A0|A1; WPQ 4: A0|A1|B0 (GATE_B0)
-      unsigned char* gbuf1 = gbuf0 + 4096;
-      // lane handles piece (lane & 7) of rows (it*4 + lane/8): source pointers / smem offsets are fixed per tile
-      const float* gptr[8];
-      uint32_t goff[8];
-#pragma unroll
-      for (int it = 0; it < 8; ++it) {
-        const int row = it * 4 + (lane >> 3), piece = lane & 7;
-        gptr[it] = P.uvab + (size_t)s_col[q * 32 + row] * 4 * H + ((piece < 4) ? 2 * H : H) + cbase + 4 * (piece & 3);
-        goff[it] = sw128_off(row, piece);
-      }
-      auto gather_issue = [&](int sub, unsigned char* buf) {
-        const uint32_t b32 = smem_u32(buf);
-#pragma unroll
-        for (int it = 0; it < 8; ++it) cp_async16(b32 + goff[it], gptr[it] + sub * 16);
-        cp_async_commit();
-      };
-      constexpr int NSUB = Cfg::CPP / 16;
-      gather_issue(0, gbuf0);
-      gather_issue(1, gbuf1);
-      const float4* pb = reinterpret_cast<const float4*>(uv_row + 3 * H + cbase);
-      uint32_t vn[16];
-      float4 bn[4];
-      if constexpr (Cfg::PREFETCH) tmem_ld16(t_acc1 + cbase, vn);
-      if constexpr (Cfg::PREFETCH) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) bn[j] = __ldg(pb + j);
-      }
-      float2 nK = splat2(0.f), S1p = splat2(0.f), S1q = splat2(0.f), Q1p = splat2(0.f), Q1q = splat2(0.f);
-      constexpr int PC = Cfg::PATCH_COLS;
-#pragma unroll 1
-      for (int sub = 0; sub < NSUB; ++sub) {
-        const int c0 = cbase + sub * 16;
-        unsigned char* buf = (sub & 1) ? gbuf1 : gbuf0;
-        uint32_t v[16];
-        float4 bb[4];
-        PROF_SUB_START();
-        if constexpr (Cfg::PREFETCH) {
-          tmem_wait_ld();
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = vn[j];
-          if (sub + 1 < NSUB) tmem_ld16(t_acc1 + c0 + 16, vn);
-        } else {
-          tmem_ld16(t_acc1 + c0, v);
-        }
-        if constexpr (Cfg::PREFETCH) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) bb[j] = bn[j];
-          if (sub + 1 < NSUB) {             // B h[row] of the next sub-chunk: an L2 round trip hidden behind this one
-#pragma unroll
-            for (int j = 0; j < 4; ++j) bn[j] = __ldg(pb + 4 * (sub + 1) + j);
-          }
-        } else {                            // 16-warp variant: no register room for the prefetch
-#pragma unroll
-          for (int j = 0; j < 4; ++j) bb[j] = __ldg(pb + 4 * sub + j);
-          tmem_wait_ld();
-        }
-        SUBPH(8);                           // tmem wait + prefetch issue
-        if (sub + 1 < NSUB) cp_async_wait<1>(); else cp_async_wait<0>();
-        __syncwarp();                       // this warp's pieces of the sub-chunk have landed
-        SUBPH(9);                           // gather wait
-#pragma unroll
-        for (int ps = 0; ps < 16 / PC; ++ps) {
-#pragma unroll
-          for (int jj = 0; jj < PC / 4; ++jj) {
-            const int j = ps * (PC / 4) + jj;
-            float4 a, vv;
-#ifdef DFB_PHASE_PROF
-            if (P.probe & 1) { a = vv = make_float4(0.1f, 0.2f, 0.3f, 0.4f); }   // tuning build: time E1 without its gather data
-            else
-#endif
-            {
-              a = *reinterpret_cast<const float4*>(buf + sw128_off(lane, j));
-              vv = *reinterpret_cast<const float4*>(buf + sw128_off(lane, 4 + j));
-            }
-            const float4 b = bb[j];
-            float2 x01 = add2(add2(make_float2(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1])),
-                                   make_float2(a.x, a.y)), make_float2(b.x, b.y));
-            float2 x23 = add2(add2(make_float2(__uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3])),
-                                   make_float2(a.z, a.w)), make_float2(b.z, b.w));
-            if (sub == 0 && j == 0) nK = splat2(-x01.x);
-            const float2 d01 = add2(x01, nK), d23 = add2(x23, nK);
-            S1p = add2(S1p, d01);
-            S1q = add2(S1q, d23);
-            Q1p = fma2(d01, d01, Q1p);
-            Q1q = fma2(d23, d23, Q1q);
-            float2 m01 = mul2(sigmoid_mufu2(x01), make_float2(vv.x, vv.y));
-            float2 m23 = mul2(sigmoid_mufu2(x23), make_float2(vv.z, vv.w));
-            if (!valid) m01 = m23 = splat2((P.agg_mode == AGG_MAX) ? -INFINITY : 0.0f);
-            patch[(4 * jj + 0) * 36 + lane] = m01.x;   // transposed [column][row]: conflict-free (4c + lane)
-            patch[(4 * jj + 1) * 36 + lane] = m01.y;
-            patch[(4 * jj + 2) * 36 + lane] = m23.x;
-            patch[(4 * jj + 3) * 36 + lane] = m23.y;
-            v[4 * j] = __float_as_uint(x01.x);
-            v[4 * j + 1] = __float_as_uint(x01.y);
-            v[4 * j + 2] = __float_as_uint(x23.x);
-            v[4 * j + 3] = __float_as_uint(x23.y);
-          }
-          __syncwarp();                     // patch pass complete
-          // row-segment reduction: lane = (column = lane % PC, row group = lane / PC) sums its PC rows of every node
-          // segment from the transposed patch; row groups are combined with shuffles; seg_mask is warp-uniform;
-          // partial rows leave as coalesced stores
-          {
-            const float* pcol = patch + (lane % PC) * 36;
-            const int r_lo = (lane / PC) * PC, r_hi = r_lo + PC - 1;
-            float mv[PC];
-#pragma unroll
-            for (int j4 = 0; j4 < PC / 4; ++j4) {
-              const float4 t4 = *reinterpret_cast<const float4*>(pcol + r_lo + 4 * j4);
-              mv[4 * j4] = t4.x; mv[4 * j4 + 1] = t4.y; mv[4 * j4 + 2] = t4.z; mv[4 * j4 + 3] = t4.w;
-            }
-            uint32_t mask = seg_mask;
-            int start = 0;
-            while (mask) {                         // one iteration per node segment present in this warp
-              const int end = __ffs(mask) - 1;
-              mask &= mask - 1;
-              const int lo = max(start, r_lo) - r_lo, hi = min(end, r_hi) - r_lo;   // my PC rows of this segment
-              const uint32_t rm = (hi >= lo) ? (((2u << hi) - 1u) & ~((1u << lo) - 1u)) : 0u;
-              float run;
-              if (P.agg_mode == AGG_MAX) {
-                float r0 = -INFINITY, r1 = -INFINITY;
-#pragma unroll
-                for (int i = 0; i < PC; i += 2) {
-                  if ((rm >> i) & 1u) r0 = fmaxf(r0, mv[i]);
-                  if ((rm >> (i + 1)) & 1u) r1 = fmaxf(r1, mv[i + 1]);
-                }
-                run = fmaxf(r0, r1);
-#pragma unroll
-                for (int off = PC; off < 32; off <<= 1) run = fmaxf(run, __shfl_xor_sync(0xffffffffu, run, off));
-              } else {
-                float r0 = 0.f, r1 = 0.f, r2 = 0.f, r3 = 0.f;
-#pragma unroll
-                for (int i = 0; i < PC; i += 4) {
-                  if ((rm >> i) & 1u) r0 += mv[i];
-                  if ((rm >> (i + 1)) & 1u) r1 += mv[i + 1];
-                  if ((rm >> (i + 2)) & 1u) r2 += mv[i + 2];
-                  if ((rm >> (i + 3)) & 1u) r3 += mv[i + 3];
-                }
-                run = (r0 + r1) + (r2 + r3);
-#pragma unroll
-                for (int off = PC; off < 32; off <<= 1) run += __shfl_xor_sync(0xffffffffu, run, off);   // fixed tree
-              }
-              if (lane < PC) {
-                const int node = s_row[q * 32 + end];
-                P.partials[(pair_base + (size_t)(node - first_node)) * H + c0 + ps * PC + lane] = run;
-              }
-              start = end + 1;
-            }
-          }
-          __syncwarp();                     // patch may be rewritten
-        }
-        if (P.write_e) tmem_st16(t_acc1 + c0, v);
-        SUBPH(10);                          // math + segment reduce
-        if (sub + 2 < NSUB) gather_issue(sub + 2, buf);
-        SUBPH(11);                          // gather issue
-      }
-      const float K1 = -nK.x, S1 = (S1p.x + S1p.y) + (S1q.x + S1q.y), Q1 = (Q1p.x + Q1p.y) + (Q1q.x + Q1q.y);
-      if (!P.write_e) {   // MIS last layer: edge stream is dead (gnn_encoder.py:412)
-        tmem_wait_ld();
-        tc_fence_before();
-        // every warp must have left E1 before the next tile's setup overwrites s_row / s_col (read by E1's gather
-        // setup and segment flush); with GATE_B0 this also marks the gather buffers in B0 dead
-        worker_bar();
-        if (wt == 0) mbar_arrive(e1_done);
-        continue;
-      }
-      tmem_wait_st();
-      float mean1, rstd1;
-      // LayerNorm statistics of the column parts are exchanged through the (now idle) per-warp patches:
-      // warp (part, q) publishes its 32 rows at patch[0..95] (K,S,Q) and patch[128..191] (S2,Q2)
-      if constexpr (WPQ == 1) {
-        worker_bar();   // every warp is done with its gather buffers
-        if (wt == 0) mbar_arrive(e1_done);
-        mean1 = K1 + S1 * (1.0f / H);
-        const float var1 = fmaxf(Q1 * (1.0f / H) - (S1 * (1.0f / H)) * (S1 * (1.0f / H)), 0.0f);
-        rstd1 = rsqrtf(var1 + LN_EPS);
-      } else {
-        patch[lane] = K1;
-        patch[32 + lane] = S1;
-        patch[64 + lane] = Q1;
-        worker_bar();
-        if (wt == 0) mbar_arrive(e1_done);   // gather buffers are dead: residual boxes / GEMM2's weights may land
-        float kk[WPQ], sp[WPQ], qp[WPQ];
-        float msum = 0.f;
-#pragma unroll
-        for (int p2 = 0; p2 < WPQ; ++p2) {
-          const float* pp = patch_all + (p2 * 4 + ((warp - 2) & 3)) * Cfg::PATCH_COLS * 36;
-          kk[p2] = pp[lane]; sp[p2] = pp[32 + lane]; qp[p2] = pp[64 + lane];
-          msum += kk[p2] * (float)Cfg::CPP + sp[p2];
-        }
-        mean1 = msum * (1.0f / H);
-        float ss = 0.f;   // sum (x - mean)^2 = sum_p [Q_p - 2 (mean - K_p) S_p + n_p (mean - K_p)^2]
-#pragma unroll
-        for (int p2 = 0; p2 < WPQ; ++p2) {
-          const float dk = mean1 - kk[p2];
-          ss += qp[p2] - 2.0f * dk * sp[p2] + (float)Cfg::CPP * dk * dk;
-        }
-        rstd1 = rsqrtf(fmaxf(ss * (1.0f / H), 0.0f) + LN_EPS);
-      }
-      PHASE(2);   // E1 (+ stats exchange)
-      // ---------------- E2: e_til = relu(LN_e(e_hat)) + tau, statistics for LN_O ----------------
-      float S2, Q2;   // e_til = relu(.)+tau is O(1) with mean ~ std: plain sums are safe in fp32
-      {
-        const float2 rs = splat2(rstd1), nm = splat2(-mean1 * rstd1);
-        float2 S2p = splat2(0.f), Q2p = splat2(0.f);
-#pragma unroll 1
-        for (int c0 = cbase; c0 < cbase + Cfg::CPP; c0 += Cfg::CW) {
-          uint32_t v[Cfg::CW];
-          tmem_ldN<Cfg::CW>(t_acc1 + c0, v);
-          tmem_wait_ld();
-#pragma unroll
-          for (int j = 0; j < Cfg::CW / 4; ++j) {
-            const float4 g4 = *reinterpret_cast<const float4*>(prm + c0 + 4 * j);
-            const float4 b4 = *reinterpret_cast<const float4*>(prm + H + c0 + 4 * j);
-            const float4 t4 = *reinterpret_cast<const float4*>(prm + 2 * H + c0 + 4 * j);
-#pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-              const float2 x = make_float2(__uint_as_float(v[4 * j + 2 * hh]), __uint_as_float(v[4 * j + 2 * hh + 1]));
-              const float2 gg = hh ? make_float2(g4.z, g4.w) : make_float2(g4.x, g4.y);
-              const float2 bb2 = hh ? make_float2(b4.z, b4.w) : make_float2(b4.x, b4.y);
-              const float2 tt = hh ? make_float2(t4.z, t4.w) : make_float2(t4.x, t4.y);
-              float2 y = fma2(fma2(x, rs, nm), gg, bb2);          // LN_e affine
-              y = add2(make_float2(fmaxf(y.x, 0.0f), fmaxf(y.y, 0.0f)), tt);   // ReLU + time vector
-              S2p = add2(S2p, y);
-              Q2p = fma2(y, y, Q2p);
-              v[4 * j + 2 * hh] = __float_as_uint(y.x);
-              v[4 * j + 2 * hh + 1] = __float_as_uint(y.y);
-            }
-          }
-          tmem_stN<Cfg::CW>(t_acc1 + c0, v);
-        }
-        S2 = S2p.x + S2p.y;
-        Q2 = Q2p.x + Q2p.y;
-      }
-      tmem_wait_st();
-      if constexpr (WPQ > 1) {
-        patch[128 + lane] = S2;
-        patch[160 + lane] = Q2;
-        worker_bar();
-        S2 = 0.f;
-        Q2 = 0.f;
-#pragma unroll
-        for (int p2 = 0; p2 < WPQ; ++p2) {
-          const float* pp = patch_all + (p2 * 4 + ((warp - 2) & 3)) * Cfg::PATCH_COLS * 36;
-          S2 += pp[128 + lane];
-          Q2 += pp[160 + lane];
-        }
-      }
-      const float mean2 = S2 * (1.0f / H);
-      const float var2 = fmaxf(Q2 * (1.0f / H) - mean2 * mean2, 0.0f);
-      const float rstd2 = rsqrtf(var2 + LN_EPS);
-      const float2 rs2 = splat2(rstd2), nm2 = splat2(-mean2 * rstd2);
-
-      PHASE(3);   // E2
-      // ---------------- E3: s = silu(LN_O(e_til)) -> GEMM2 A operand chunks (this part's K-chunks) ----------------
-#pragma unroll 1
-      // every K-chunk (64 columns of s) is produced cooperatively: part p converts columns [64 kc + p*64/WPQ, +64/WPQ),
-      // so chunk 0 is complete after 1/4 of E3 and GEMM2 runs underneath the rest of E3
-      for (int kc = 0; kc < 4; ++kc) {
-#pragma unroll 1
-        for (int piece = 0; piece < (TC_KCH / WPQ) / Cfg::CW; ++piece) {
-          const int cc = part * (TC_KCH / WPQ) + piece * Cfg::CW;   // column offset inside the 64-column chunk
-          const int c0 = kc * TC_KCH + cc;
-          uint32_t v[Cfg::CW];
-          tmem_ldN<Cfg::CW>(t_acc1 + c0, v);
-          tmem_wait_ld();
-#pragma unroll
-          for (int g16 = 0; g16 < Cfg::CW / 16; ++g16) {   // one MMA k-step (16 elements) = 8 columns hi + 8 columns lo
-            uint32_t w16[16];
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {               // 8 elements each
-              float z[8];
-#pragma unroll
-              for (int hh = 0; hh < 2; ++hh) {
-                const int e0 = 16 * g16 + 8 * j + 4 * hh;
-                const float4 g4 = *reinterpret_cast<const float4*>(prm + 3 * H + c0 + e0);
-                const float4 b4 = *reinterpret_cast<const float4*>(prm + 4 * H + c0 + e0);
-                const float2 t01 = fma2(fma2(make_float2(__uint_as_float(v[e0]), __uint_as_float(v[e0 + 1])), rs2, nm2),
-                                        make_float2(g4.x, g4.y), make_float2(b4.x, b4.y));
-                const float2 t23 = fma2(fma2(make_float2(__uint_as_float(v[e0 + 2]), __uint_as_float(v[e0 + 3])), rs2, nm2),
-                                        make_float2(g4.z, g4.w), make_float2(b4.z, b4.w));
-                const float2 s01 = mul2(t01, sigmoid_mufu2(t01)), s23 = mul2(t23, sigmoid_mufu2(t23));   // SiLU
-                z[4 * hh] = s01.x; z[4 * hh + 1] = s01.y; z[4 * hh + 2] = s23.x; z[4 * hh + 3] = s23.y;
-              }
-              uint2 h0, l0, h1, l1;
-              split4(make_float4(z[0], z[1], z[2], z[3]), h0, l0);
-              split4(make_float4(z[4], z[5], z[6], z[7]), h1, l1);
-              w16[4 * j] = h0.x; w16[4 * j + 1] = h0.y; w16[4 * j + 2] = h1.x; w16[4 * j + 3] = h1.y;             // hi: columns 0..7
-              w16[8 + 4 * j] = l0.x; w16[8 + 4 * j + 1] = l0.y; w16[8 + 4 * j + 2] = l1.x; w16[8 + 4 * j + 3] = l1.y;   // lo: columns 8..15
-            }
-            tmem_st16(t_acc1 + c0 + 16 * g16, w16);
-          }
-        }
-        tmem_wait_st();
-        tc_fence_before();
-        mbar_arrive(&full_a2[kc]);
-      }
-
-      PHASE(4);   // E3
-      // ---------------- E4: e = e_in + O(s) + b_O (this part's columns) ----------------
-      mbar_wait(&acc_rdy[1], tile_par, P.error_flag, 7);
-      tc_fence_after();
-      PHASE(5);   // wait for GEMM2
-      {
-        // All MMAs of the tile are complete: the operand area is idle.  The fp32 residual tile comes in by
-        // TMA (8 boxes of [128 rows x 32 cols], 128B swizzle -> conflict-free thread==row access), the result
-        // (issued by the producer warp while E3 / GEMM2 were still running), the result is written over it and leaves
-        // by TMA store: no uncoalesced global access, e read from L2 once more.
-        const bool tma_in = !P.e_zero && !P.xt_lut;
-        if (tma_in) mbar_wait(ein_bar, tile_par, P.error_flag, 10);   // issued early by the producer warp
-#pragma unroll 1
-        for (int c0 = cbase; c0 < cbase + Cfg::CPP; c0 += Cfg::CW) {
-          uint32_t v[Cfg::CW];
-          tmem_ldN<Cfg::CW>(t_acc2 + c0, v);
-          tmem_wait_ld();
-          unsigned char* box = smem + (c0 >> 5) * TC_BOX_BYTES;
-          const int u0 = (c0 & 31) >> 2;   // first 16-byte unit of this chunk inside its 32-column box
-#pragma unroll
-          for (int j = 0; j < Cfg::CW / 4; ++j) {
-            float4* slot = reinterpret_cast<float4*>(box + sw128_off(r, u0 + j));
-            const float4 ein = tma_in ? *slot : __ldg(reinterpret_cast<const float4*>(src + c0) + j);
-            const float4 bo = *reinterpret_cast<const float4*>(prm + 5 * H + c0 + 4 * j);
-            const float2 o01 = add2(add2(make_float2(ein.x, ein.y), make_float2(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]))),
-                                    make_float2(bo.x, bo.y));
-            const float2 o23 = add2(add2(make_float2(ein.z, ein.w), make_float2(__uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]))),
-                                    make_float2(bo.z, bo.w));
-            const float4 o = make_float4(o01.x, o01.y, o23.x, o23.y);
-            *slot = o;
-          }
-        }
-        fence_proxy_async();   // generic-proxy smem writes -> visible to the TMA store
-        tc_fence_before();
-        worker_bar();
-        if (wt == 0) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) tma_store_2d(&emap, smem_base + j * TC_BOX_BYTES, 32 * j, tile * TC_TILE);
-          tma_store_commit();
-          tma_store_wait_read();
-          mbar_arrive(e4_done);
-        }
-      }
-      tc_fence_before();
-      PHASE(6);   // E4
+      w_row[tid] = rw;
+      w_src[tid] = src;
     }
-#ifdef DFB_PHASE_PROF
-    if (prof)
-      for (int i = 0; i < 16; ++i) atomicAdd(P.phase_cycles + i, (unsigned long long)pc[i]);
-#endif
-#undef PHASE
-#undef SUBPH
-#undef PROF_TILE_START
-#undef PROF_SUB_START
-  }
+    wg_bar();   // row table visible; every warp has left the previous tile's GEMM2 (A operand area free)
 
-  // teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+    // ---------------- GEMM1 A operand: fp32 rows -> bf16 hi/lo, K-major 128B-swizzled chunks ----------------
+#pragma unroll 4
+    for (int it = 0; it < 32; ++it) {
+      const int item = it * 128 + tid;
+      const int rr = item >> 6, k4 = item & 63;
+      const float4 x = __ldcg(reinterpret_cast<const float4*>(w_src[rr]) + k4);
+      uint2 hi, lo;
+      split4(x, hi, lo);
+      const uint32_t off = (k4 >> 4) * 2 * TC_A_CHUNK + sw128_off(rr, (k4 & 15) >> 1) + (k4 & 1) * 8;
+      *reinterpret_cast<uint2*>(a_reg + off) = hi;
+      *reinterpret_cast<uint2*>(a_reg + off + TC_A_CHUNK) = lo;
+    }
+    fence_proxy_async();   // generic-proxy stores -> visible to wgmma
+    wg_bar();
+    gemm();
+
+    const int sa = s_base + lr0, sb = sa + 8;
+    const bool va = sa < n_rows, vb = sb < n_rows;
+    if (lin || P.debug_acc) {
+      const int nb = (lin && P.lin_nb == 4) ? (tile & 3) : 0;
+      const int ostride = lin ? P.lin_nb * H : H;
+      float* out = lin ? P.lin_out + nb * H : P.debug_acc;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int s = h ? sb : sa;
+        if (!(h ? vb : va)) continue;
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          const int c = 8 * j + 2 * t4;
+          float2 o = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+          if (lin) {
+            const float2 bb = __ldg(reinterpret_cast<const float2*>(P.lin_bias + nb * H + c));
+            o.x += bb.x;
+            o.y += bb.y;
+          }
+          __stcg(reinterpret_cast<float2*>(out + (size_t)s * ostride + c), o);
+        }
+      }
+      continue;
+    }
+
+    // ---------------- E1: e_hat = acc + A h[col] + B h[row];  messages sigmoid(e_hat) * V h[col] ----------------
+    const float* src_a = w_src[lr0];
+    const float* src_b = w_src[lr0 + 8];
+    {
+      const float* col_a = P.uvab + (size_t)(va ? P.g.col[sa] : 0) * 4 * H;
+      const float* col_b = P.uvab + (size_t)(vb ? P.g.col[sb] : 0) * 4 * H;
+      const float* row_a = P.uvab + (size_t)(va ? P.g.row[sa] : 0) * 4 * H + 3 * H;
+      const float* row_b = P.uvab + (size_t)(vb ? P.g.row[sb] : 0) * 4 * H + 3 * H;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const int c = 8 * j + 2 * t4;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float* cp = h ? col_b : col_a;
+          const float2 ah = __ldg(reinterpret_cast<const float2*>(cp + 2 * H + c));
+          const float2 vh = __ldg(reinterpret_cast<const float2*>(cp + H + c));
+          const float2 bh = __ldg(reinterpret_cast<const float2*>((h ? row_b : row_a) + c));
+          const float x0 = (acc[4 * j + 2 * h] + ah.x) + bh.x;
+          const float x1 = (acc[4 * j + 2 * h + 1] + ah.y) + bh.y;
+          acc[4 * j + 2 * h] = x0;
+          acc[4 * j + 2 * h + 1] = x1;
+          const int r = lr0 + 8 * h;
+          *reinterpret_cast<float2*>(msg + r * H + (c ^ (8 * (r & 7)))) =
+              make_float2(sigmoid_mufu(x0) * vh.x, sigmoid_mufu(x1) * vh.y);
+        }
+      }
+    }
+    wg_bar();   // messages of all 64 rows are in shared memory
+    // row-segment reduction: thread = column, rows of each 32-edge group in order (the fp32 kernel's order)
+#pragma unroll 1
+    for (int g2 = 0; g2 < WG_ROWS / GROUP; ++g2) {
+      const int grp = (s_base >> 5) + g2;
+      if (grp >= P.g.n_groups) break;
+      const int first_node = P.g.grp_first[grp];
+      const size_t pair_base = (size_t)P.g.grp_pair[grp];
+#pragma unroll
+      for (int cc = 0; cc < 2; ++cc) {
+        const int c = tid + 128 * cc;
+        float run = (P.agg_mode == AGG_MAX) ? -INFINITY : 0.0f;
+#pragma unroll 4
+        for (int r = 0; r < GROUP; ++r) {
+          const int lr = g2 * GROUP + r;
+          const int node = w_row[lr];
+          if (node < 0) break;
+          const float m = msg[lr * H + (c ^ (8 * (lr & 7)))];
+          run = (P.agg_mode == AGG_MAX) ? fmaxf(run, m) : run + m;
+          const int nxt = (r + 1 < GROUP) ? w_row[lr + 1] : -1;
+          if (nxt != node) {
+            P.partials[(pair_base + (size_t)(node - first_node)) * H + c] = run;
+            run = (P.agg_mode == AGG_MAX) ? -INFINITY : 0.0f;
+          }
+        }
+      }
+    }
+    wg_bar();   // messages consumed: the area takes GEMM2's A operand next; the row table may be rewritten
+    if (!P.write_e) continue;   // MIS last layer: the edge stream is never read again (gnn_encoder.py:412)
+
+    // ---------------- E2 / E3: e_til = relu(LN_e(e_hat)) + tau;  s = silu(LN_O(e_til)) -> GEMM2 A operand ----------------
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float sum = 0.f;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) sum += acc[4 * j + 2 * h] + acc[4 * j + 2 * h + 1];
+      float mean = quad_sum(sum) * (1.0f / H);
+      float q = 0.f;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const float d0 = acc[4 * j + 2 * h] - mean, d1 = acc[4 * j + 2 * h + 1] - mean;
+        q = fmaf(d0, d0, fmaf(d1, d1, q));
+      }
+      float rstd = rsqrtf(quad_sum(q) * (1.0f / H) + LN_EPS);
+      sum = 0.f;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const int c = 8 * j + 2 * t4;
+        const float2 g = *reinterpret_cast<const float2*>(prm + c);
+        const float2 b = *reinterpret_cast<const float2*>(prm + H + c);
+        const float2 t = *reinterpret_cast<const float2*>(prm + 2 * H + c);
+        const float y0 = fmaxf(fmaf((acc[4 * j + 2 * h] - mean) * rstd, g.x, b.x), 0.0f) + t.x;
+        const float y1 = fmaxf(fmaf((acc[4 * j + 2 * h + 1] - mean) * rstd, g.y, b.y), 0.0f) + t.y;
+        acc[4 * j + 2 * h] = y0;
+        acc[4 * j + 2 * h + 1] = y1;
+        sum += y0 + y1;
+      }
+      mean = quad_sum(sum) * (1.0f / H);
+      q = 0.f;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const float d0 = acc[4 * j + 2 * h] - mean, d1 = acc[4 * j + 2 * h + 1] - mean;
+        q = fmaf(d0, d0, fmaf(d1, d1, q));
+      }
+      rstd = rsqrtf(quad_sum(q) * (1.0f / H) + LN_EPS);
+      const int r = lr0 + 8 * h;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const int c = 8 * j + 2 * t4;
+        const float2 g = *reinterpret_cast<const float2*>(prm + 3 * H + c);
+        const float2 b = *reinterpret_cast<const float2*>(prm + 4 * H + c);
+        const float z0 = fmaf((acc[4 * j + 2 * h] - mean) * rstd, g.x, b.x);
+        const float z1 = fmaf((acc[4 * j + 2 * h + 1] - mean) * rstd, g.y, b.y);
+        uint32_t hi, lo;
+        split2(z0 * sigmoid_mufu(z0), z1 * sigmoid_mufu(z1), hi, lo);   // SiLU
+        const uint32_t off = (j >> 3) * 2 * TC_A_CHUNK + sw128_off(r, j & 7) + 4 * t4;
+        *reinterpret_cast<uint32_t*>(a_reg + off) = hi;
+        *reinterpret_cast<uint32_t*>(a_reg + off + TC_A_CHUNK) = lo;
+      }
+    }
+    fence_proxy_async();
+    wg_bar();
+    gemm();   // GEMM2: acc = s * O^T
+
+    // ---------------- E4: e = e_in + O(s) + b_O (in place) ----------------
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (!(h ? vb : va)) continue;
+      const float* src = h ? src_b : src_a;
+      float* dst = P.e + (size_t)(h ? sb : sa) * H;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const int c = 8 * j + 2 * t4;
+        const float2 ein = __ldcg(reinterpret_cast<const float2*>(src + c));
+        const float2 bo = *reinterpret_cast<const float2*>(prm + 5 * H + c);
+        __stcg(reinterpret_cast<float2*>(dst + c),
+               make_float2((ein.x + acc[4 * j + 2 * h]) + bo.x, (ein.y + acc[4 * j + 2 * h + 1]) + bo.y));
+      }
+    }
   }
 }
 
-// Kernel entry points: one per worker-warp count.  (576 threads are allocated as 20 warps: 96 registers per thread.)
-template <int WPQ>
-__global__ void __launch_bounds__(TcCfg<WPQ>::THREADS, 1)
-k_edge_layer_tc(const __grid_constant__ CUtensorMap wmap, const __grid_constant__ CUtensorMap emap, const TcParams P) {
-  edge_layer_tc_body<WPQ>(wmap, emap, P);
+// Kernel entry points.  The two-warpgroup kernel (128-row tiles) is the product path; the one-warpgroup kernel
+// (64-row tiles, a different tiling of the same graph) is the A/B and validation variant (DFB_EDGE_IMPL_TC1).
+__global__ void __launch_bounds__(TcCfg<2>::THREADS, 1)
+k_edge_layer_wg2(const __grid_constant__ CUtensorMap wmap, const TcParams P) {
+  edge_layer_wg_body<2>(wmap, P);
 }
-__global__ void __launch_bounds__(TcCfg<4>::THREADS, 1)
-k_edge_layer_tc16w(const __grid_constant__ CUtensorMap wmap, const __grid_constant__ CUtensorMap emap, const TcParams P) {
-  edge_layer_tc_body<4>(wmap, emap, P);
+__global__ void __launch_bounds__(TcCfg<1>::THREADS, 1)
+k_edge_layer_wg1(const __grid_constant__ CUtensorMap wmap, const TcParams P) {
+  edge_layer_wg_body<1>(wmap, P);
 }
 // the same body in linear mode (node-side / embedding linears) under its own name, so launch lists and profiles
 // do not mix the two uses
-__global__ void __launch_bounds__(TcCfg<4>::THREADS, 1)
-k_linear_tc16w(const __grid_constant__ CUtensorMap wmap, const __grid_constant__ CUtensorMap emap, const TcParams P) {
-  edge_layer_tc_body<4>(wmap, emap, P);
+__global__ void __launch_bounds__(TcCfg<2>::THREADS, 1)
+k_linear_wg2(const __grid_constant__ CUtensorMap wmap, const TcParams P) {
+  edge_layer_wg_body<2>(wmap, P);
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -988,14 +521,9 @@ struct TcState {
   std::string err;
   int num_sms = 0;
   CUtensorMap wmap;
-  CUtensorMap emap;                 // fp32 edge stream [E_pad][256], box 32 cols x 128 rows, 128B swizzle
-  const void* emap_ptr = nullptr;
-  long long emap_rows = 0;
-  void* encode_fn = nullptr;
   bool bound = false;
   int last_launches = 0;
   float* zero_row = nullptr;
-  float* zero_row4 = nullptr;   // [4 * 256] zeros: a whole uvab row (pair kernel: gathers of rows past the edge list)
   int* error_flag = nullptr;    // device alias of error_host (host-mapped: readable after a trap)
   int* error_host = nullptr;
   float* debug_acc = nullptr;   // set by the debug entry point for one launch
@@ -1003,9 +531,7 @@ struct TcState {
   float* lin_out = nullptr;
   const float* lin_bias = nullptr;
   int lin_rows = 0, lin_nb = 4, lin_w_row = 0;
-  int wpq = 4;                  // worker warps per TMEM lane quarter (DFB_TC_WPQ tuning knob: 1, 2 or 4)
-  int probe = 0;                // DFB_TC_PROBE tuning knob, read once at context creation
-  unsigned long long* phase_cycles = nullptr;
+  unsigned long long* phase_cycles = nullptr;   // dfb_debug_phase_cycles: these kernels record none (stays zero)
 };
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -1014,28 +540,17 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
 
 inline int tc_init(TcState* st, int num_sms) {
   st->num_sms = num_sms;
-  cudaError_t e = cudaFuncSetAttribute(k_edge_layer_tc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<1>::SMEM_ALLOC);
+  cudaError_t e = cudaFuncSetAttribute(k_edge_layer_wg2, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<2>::SMEM_ALLOC);
   if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(k_edge_layer_tc<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<2>::SMEM_ALLOC);
+    e = cudaFuncSetAttribute(k_edge_layer_wg1, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<1>::SMEM_ALLOC);
   if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(k_edge_layer_tc16w, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<4>::SMEM_ALLOC);
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(k_linear_tc16w, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<4>::SMEM_ALLOC);
+    e = cudaFuncSetAttribute(k_linear_wg2, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<2>::SMEM_ALLOC);
   if (e != cudaSuccess) {
     st->err = std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e);
     return -2;
   }
-  {
-    const char* w = getenv("DFB_TC_WPQ");
-    st->wpq = w ? atoi(w) : 4;
-    if (st->wpq != 1 && st->wpq != 2 && st->wpq != 4) st->wpq = 4;
-    const char* pe = getenv("DFB_TC_PROBE");
-    st->probe = pe ? atoi(pe) : 0;
-  }
   if ((e = cudaMalloc(&st->zero_row, H * sizeof(float))) != cudaSuccess ||
       (e = cudaMemset(st->zero_row, 0, H * sizeof(float))) != cudaSuccess ||
-      (e = cudaMalloc(&st->zero_row4, 4 * H * sizeof(float))) != cudaSuccess ||
-      (e = cudaMemset(st->zero_row4, 0, 4 * H * sizeof(float))) != cudaSuccess ||
       (e = cudaMalloc(&st->phase_cycles, 32 * sizeof(unsigned long long))) != cudaSuccess ||
       (e = cudaMemset(st->phase_cycles, 0, 32 * sizeof(unsigned long long))) != cudaSuccess ||
       (e = cudaHostAlloc(&st->error_host, 4 * sizeof(int), cudaHostAllocMapped)) != cudaSuccess ||
@@ -1048,7 +563,6 @@ inline int tc_init(TcState* st, int num_sms) {
 
 inline void tc_destroy(TcState* st) {
   if (st->zero_row) cudaFree(st->zero_row);
-  if (st->zero_row4) cudaFree(st->zero_row4);
   if (st->error_host) cudaFreeHost(st->error_host);
   if (st->phase_cycles) cudaFree(st->phase_cycles);
   st->zero_row = nullptr;
@@ -1079,62 +593,35 @@ inline int tc_bind_weights(TcState* st, const LayerParams* layers, int L) {
     st->err = "cuTensorMapEncodeTiled failed with CUresult " + std::to_string((int)r);
     return -2;
   }
-  st->encode_fn = fn;
   st->bound = true;
   return 0;
 }
 
-// fp32 edge stream [E_pad][256] as a 2-D tensor map: box 32 columns x 128 rows, 128-byte swizzle (re-encoded only when
-// the buffer or its size changes)
-inline int tc_ensure_emap(TcState* st, const float* e, int E) {
-  const long long e_rows = (long long)((E + TC_TILE - 1) / TC_TILE) * TC_TILE;
-  if (st->emap_ptr == (const void*)e && st->emap_rows == e_rows) return 0;
-  cuuint64_t gdim[2] = {(cuuint64_t)H, (cuuint64_t)e_rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)H * sizeof(float)};
-  cuuint32_t box[2] = {32u, (cuuint32_t)TC_TILE};
-  cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = ((PFN_encodeTiled)st->encode_fn)(&st->emap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)e, gdim, gstride,
-                                                box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    st->err = "cuTensorMapEncodeTiled(e) failed with CUresult " + std::to_string((int)r);
-    return -2;
-  }
-  st->emap_ptr = (const void*)e;
-  st->emap_rows = e_rows;
-  return 0;
-}
-
+// nwg: consumer warpgroups per CTA (2: product kernel, 1: the 64-row-tile variant)
 inline int tc_launch_edge_layer(TcState* st, int l, float* e, const float* uvab, float* partials, GraphDev g,
                                 LayerParams lp, const float* tvec_edge, int write_e, int e_zero,
-                                const float* xt_lut, const float* lut, int agg_mode, cudaStream_t stream) {
+                                const float* xt_lut, const float* lut, int agg_mode, cudaStream_t stream, int nwg = 2) {
   st->last_launches = 0;
   if (!st->bound) {
     st->err = "weights not bound";
     return -1;
   }
-  if (!st->lin_out) {   // linear mode never touches the edge stream
-    int r = tc_ensure_emap(st, e, g.E);
-    if (r) return r;
-  }
+  if (st->lin_out) nwg = 2;
+  const int tile_rows = nwg * WG_ROWS;
   TcParams P;
   P.e = e; P.uvab = uvab; P.partials = partials; P.g = g; P.lp = lp; P.tvec = tvec_edge;
   P.xt_lut = xt_lut; P.lut = lut; P.zero_row = st->zero_row; P.debug_acc = st->debug_acc;
   P.error_flag = st->error_flag;
-  P.phase_cycles = st->phase_cycles;
-  P.write_e = st->debug_acc ? 0 : write_e;
+  P.write_e = (st->debug_acc || st->lin_out) ? 0 : write_e;
   P.e_zero = e_zero; P.agg_mode = agg_mode;
   P.w_row_base = l * 12 * H;
   P.lin_in = st->lin_in; P.lin_out = st->lin_out; P.lin_bias = st->lin_bias; P.lin_rows = st->lin_rows;
   P.lin_nb = st->lin_nb; P.lin_w_row = st->lin_w_row;
-  P.n_tiles = st->lin_out ? st->lin_nb * ((st->lin_rows + TC_TILE - 1) / TC_TILE) : (g.E + TC_TILE - 1) / TC_TILE;
-  if (st->lin_out) P.write_e = 0;
-  P.probe = st->probe;
-  int grid = P.n_tiles < st->num_sms ? P.n_tiles : st->num_sms;
-  if (st->wpq == 1) k_edge_layer_tc<1><<<grid, TcCfg<1>::THREADS, TcCfg<1>::SMEM_ALLOC, stream>>>(st->wmap, st->emap, P);
-  else if (st->wpq == 4 && st->lin_out) k_linear_tc16w<<<grid, TcCfg<4>::THREADS, TcCfg<4>::SMEM_ALLOC, stream>>>(st->wmap, st->emap, P);
-  else if (st->wpq == 4) k_edge_layer_tc16w<<<grid, TcCfg<4>::THREADS, TcCfg<4>::SMEM_ALLOC, stream>>>(st->wmap, st->emap, P);
-  else k_edge_layer_tc<2><<<grid, TcCfg<2>::THREADS, TcCfg<2>::SMEM_ALLOC, stream>>>(st->wmap, st->emap, P);
+  P.n_tiles = st->lin_out ? st->lin_nb * ((st->lin_rows + tile_rows - 1) / tile_rows) : (g.E + tile_rows - 1) / tile_rows;
+  const int grid = P.n_tiles < st->num_sms ? P.n_tiles : st->num_sms;
+  if (st->lin_out) k_linear_wg2<<<grid, TcCfg<2>::THREADS, TcCfg<2>::SMEM_ALLOC, stream>>>(st->wmap, P);
+  else if (nwg == 1) k_edge_layer_wg1<<<grid, TcCfg<1>::THREADS, TcCfg<1>::SMEM_ALLOC, stream>>>(st->wmap, P);
+  else k_edge_layer_wg2<<<grid, TcCfg<2>::THREADS, TcCfg<2>::SMEM_ALLOC, stream>>>(st->wmap, P);
   cudaError_t err = cudaGetLastError();
   if (err != cudaSuccess) {
     st->err = std::string("launch: ") + cudaGetErrorString(err);

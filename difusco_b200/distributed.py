@@ -1,7 +1,7 @@
 """Instance-parallel sharding of the denoise path across GPUs (SURVEY 8e).
 
 The reference shards its test set over DDP ranks with batch size 1 (train.py:106-115,
-pl_meta_model.py:194-198): instances never interact, so the B200 path is one process per GPU,
+pl_meta_model.py:194-198): instances never interact, so the GPU path is one process per GPU,
 each owning a contiguous block of instances, NO collective inside the 50-step loop, and one
 all_gather of the final heatmaps at the end (north_star).  Works with the nccl backend on GPUs and
 with gloo on CPU tensors (tests/test_distributed_cpu.py).

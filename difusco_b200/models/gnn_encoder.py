@@ -4,7 +4,7 @@ Same constructor signature, same parameter tree (so `state_dict()` keys and shap
 and Lightning checkpoints load with `load_state_dict`), same `forward(x, timesteps, graph,
 edge_index)` contract (difusco/models/gnn_encoder.py:290-462) - but `forward` does no PyTorch
 math: it hands raw device pointers to the sm_100a CUDA library through the C-ABI
-(include/difusco_b200.h).  There is no eager fallback: without the library or without a B200
+(include/difusco_b200.h).  There is no eager fallback: without the library or without an H100
 the call raises.
 
 Interface notes (reference behaviour kept):

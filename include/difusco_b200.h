@@ -1,9 +1,9 @@
-/* difusco_b200 - C-ABI of the B200-native DIFUSCO denoising-inference hot path.
+/* difusco_b200 - C-ABI of the H100-native (sm_90a) DIFUSCO denoising-inference hot path.
  *
  * The reference (Edward-Sun/DIFUSCO) has no FFI / plugin interface of its own: its seams are Python
  * methods.  This header is the boundary the Python host mirror (difusco_b200/*.py) binds with
  * ctypes; every entry point names the reference interface whose device work it replaces
- * (paths relative to /root/reference/difusco).  Plain C types only; pointers are raw host or
+ * (paths relative to the reference's difusco/ directory).  Plain C types only; pointers are raw host or
  * device pointers as stated; `stream` is a cudaStream_t passed as void*.  Every function returns
  * 0 on success or a negative DFB_E_* code; dfb_last_error() gives the message.  Nothing throws
  * across the boundary.  A context is bound to one device and is not thread-safe (one per GPU /
@@ -37,8 +37,8 @@ enum {
 
 enum { DFB_TASK_TSP = 0, DFB_TASK_MIS = 1 };               /* pl_tsp_model.py / pl_mis_model.py          */
 enum { DFB_DIFFUSION_CATEGORICAL = 0, DFB_DIFFUSION_GAUSSIAN = 1 }; /* pl_meta_model.py:27-36           */
-enum { DFB_EDGE_IMPL_TC = 0, DFB_EDGE_IMPL_FP32 = 1, DFB_EDGE_IMPL_TC1 = 2 }; /* tcgen05 product path (CTA-pair kernel on the
-  middle layers) / fp32 validation kernel / the single-CTA tcgen05 kernel on every layer (A/B and validation) */
+enum { DFB_EDGE_IMPL_TC = 0, DFB_EDGE_IMPL_FP32 = 1, DFB_EDGE_IMPL_TC1 = 2 }; /* wgmma product path (128-row tiles, two
+  consumer warpgroups) / fp32 validation kernel / the wgmma kernel with 64-row tiles, one warpgroup (A/B and validation) */
 
 typedef struct dfb_ctx dfb_ctx;
 
@@ -46,8 +46,7 @@ int dfb_abi_version(void);
 
 /* Create a context on CUDA device `device`.  Fails (DFB_E_CUDA) when no device is present:
  * there is no CPU fallback.  The environment is read here and nowhere else (A/B switches, all default to the product
- * path): DFB_GRAPH_CAPTURE=0 plain launches instead of the captured loop, DFB_PAIR_KERNEL=0 single-CTA edge kernel for
- * every layer, DFB_SERPENTINE=0 every layer sweeps the edge stream upwards, DFB_TC_PROBE tuning-build counters. */
+ * path): DFB_GRAPH_CAPTURE=0 plain launches instead of the captured loop. */
 int dfb_create(dfb_ctx** out, int device);
 int dfb_destroy(dfb_ctx* ctx);
 /* Message of the last failure on `ctx` (or of the last failed dfb_create when ctx == NULL). */
@@ -177,12 +176,11 @@ int dfb_profile_end(dfb_ctx* ctx, double* edge_kernel_ms, int64_t* edge_kernel_l
  * acc_out (E,256).  DEVICE pointers.  Used by the parity tests to localise failures. */
 int dfb_debug_edge_gemm(dfb_ctx* ctx, int layer, const float* e_in, float* acc_out, void* stream);
 
-/* Tuning hook: per-phase cycle counters of the tcgen05 edge kernels (DFB_TC_PROBE bit 7, --prof build); out must hold
- * 32 unsigned 64-bit values (host): [0..7] phases and [8..15] E1 sub-phases of the single-CTA kernel, [16..23] phases of
- * the CTA-pair kernel.  Read-and-reset. */
+/* Tuning hook: per-phase cycle counters of the edge kernels; out must hold 32 unsigned 64-bit values (host).  The wgmma
+ * kernels record none: the values read back as zero.  Read-and-reset. */
 int dfb_debug_phase_cycles(dfb_ctx* ctx, unsigned long long* out);
 
-/* Diagnostic: watchdog record of the tcgen05 kernel's bounded barrier waits (host-mapped memory, readable after a
+/* Diagnostic: watchdog record of the tensor-core kernel's bounded barrier waits (host-mapped memory, readable after a
  * launch failure): out[4] = {wait-site code or 0, blockIdx.x, parity, threadIdx.x}. */
 int dfb_debug_watchdog(dfb_ctx* ctx, int* out);
 

@@ -404,6 +404,22 @@ def gen_mcts_txt():
   save("mcts_txt", **out)
 
 
+# ------------------------------------------------------------------------------------------
+def gen_ref_copy():
+  """What tests/test_reference_copy.py checks oracle/_ref against: the sha256 of every file oracle/make_ref.py copies
+  and the reference encoder's output on the test's tiny TSP instance."""
+  import hashlib
+  sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(HERE)), "oracle"))
+  import make_ref
+  sha = [hashlib.sha256(open(os.path.join(make_ref.SRC, rel), "rb").read()).hexdigest() for rel in make_ref.FILES]
+  torch.manual_seed(0)
+  w = syn.make_encoder_weights(0, out_channels=2)
+  pts, ei = syn.tsp_sparse_batch(30, 7, 2, seed=5)
+  xt = (syn.initial_noise(ei.shape[1], 3) > 0).astype(np.float32)
+  out = ref_encoder(w, 2, False)(torch.from_numpy(pts), torch.tensor([321.0]), torch.from_numpy(xt), torch.from_numpy(ei))
+  save("ref_copy", files=np.array(make_ref.FILES), sha256=np.array(sha), out=out.numpy())
+
+
 if __name__ == "__main__":
   ap = argparse.ArgumentParser()
   ap.add_argument("--only", default="")
@@ -420,3 +436,5 @@ if __name__ == "__main__":
     gen_tsp_decode()
   if a.only in ("", "mcts_txt"):
     gen_mcts_txt()
+  if a.only in ("", "ref_copy"):
+    gen_ref_copy()

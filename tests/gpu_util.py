@@ -1,4 +1,4 @@
-"""Helpers for the -m gpu parity tests (run on the B200 box; never touch /root/reference)."""
+"""Helpers for the -m gpu parity tests (run on an H100; they read nothing outside the repository)."""
 from types import SimpleNamespace as NS
 
 import numpy as np
@@ -10,7 +10,7 @@ from difusco_b200.pl_mis_model import MISModel
 from difusco_b200.pl_tsp_model import TSPModel
 
 IMPLS = {"tc": _cabi.EDGE_IMPL_TC, "fp32": _cabi.EDGE_IMPL_FP32, "tc1": _cabi.EDGE_IMPL_TC1}
-# fp32 validation kernel: fp32 reassociation only.  tcgen05 kernel: 3-term bf16 split (~2^-17 per product).
+# fp32 validation kernel: fp32 reassociation only.  wgmma kernels: 3-term bf16 split (~2^-17 per product).
 TOL = {"fp32": 2e-5, "tc": 1e-4, "tc1": 1e-4}
 
 

@@ -1,5 +1,5 @@
 """bench.py's host-side contract, checked without a GPU: the algorithmic-byte formulas (SURVEY 8d), the config table
-(BASELINE.json configs), the committed ncu traffic number, and the failure mode of the GPU arm on a box without a GPU."""
+(BASELINE.json configs), --dump-outputs on the command line, and the failure mode of the GPU arm on a machine without a GPU."""
 import json
 import os
 import subprocess
@@ -17,10 +17,11 @@ def test_algorithmic_bytes_match_survey_8d():
   assert bench.algorithmic_bytes_per_step(dict(node_only=False, E=E, V=V)) == 24576 * E          # 2 L E H 4
   mis = bench.algorithmic_bytes_per_step(dict(node_only=True, E=E, V=V))
   assert mis == (2 * 12 - 2) * E * 256 * 4 + 2 * 12 * V * 256 * 4
-  # per TSP-500 graph (E = 25 000, 50 steps): 30.72 GB -> the 213.8 graphs/s ceiling DESIGN.md quotes at 6567.7 GB/s
+  # per TSP-500 graph (E = 25 000, 50 steps): 30.72 GB -> the 109.0 graphs/s ceiling DESIGN.md quotes at the H100 SXM's
+  # 3.35 TB/s (data sheet)
   per_graph = 24576 * 25000 * 50
   assert abs(per_graph / 1e9 - 30.72) < 1e-9
-  assert abs(6567.7e9 / per_graph - 213.8) < 0.05
+  assert abs(3350e9 / per_graph - 109.0) < 0.05
 
 
 def test_config_table_covers_baseline_configs():
@@ -34,13 +35,6 @@ def test_config_table_covers_baseline_configs():
   assert wl["global_batch"] == 16 * 8 and "model" not in wl
 
 
-def test_committed_ncu_traffic_is_close_to_the_algorithmic_bytes():
-  t = bench.ncu_traffic()
-  assert t is not None
-  algo = 24576 * 400000
-  assert 1.0 <= t / algo < 1.25          # DRAM bytes of a whole step: no wasted re-reads
-
-
 def test_small_workloads_build_on_cpu():
   for name in ("C1", "B1"):
     wl = bench.build_workload(bench.CONFIGS[name], rank=0)
@@ -52,7 +46,9 @@ def test_gpu_arm_fails_loudly_without_a_gpu():
   import torch
   if torch.cuda.is_available():
     return
-  r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--steps", "1", "--warmup", "0", "--no-cpu-baseline"],
+  r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--steps", "1", "--warmup", "0", "--no-cpu-baseline",
+                      "--dump-outputs", os.path.join(ROOT, "nonexistent-dump-dir")],
                      stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600)
   assert r.returncode != 0          # no CPU fallback: the product path needs the CUDA library and a device
   assert "graphs/s" not in r.stdout.splitlines()[-1] if r.stdout.strip() else True
+  assert "unrecognized arguments" not in r.stdout and not os.path.exists(os.path.join(ROOT, "nonexistent-dump-dir"))

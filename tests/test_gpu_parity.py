@@ -1,5 +1,5 @@
 """Parity of the CUDA path (through the C-ABI) against the committed reference outputs
-(tests/golden) and against the CPU oracle on fresh seeded inputs.  Run with -m gpu on a B200."""
+(tests/golden) and against the CPU oracle on fresh seeded inputs.  Run with -m gpu on an H100."""
 import numpy as np
 import pytest
 import torch
@@ -13,7 +13,7 @@ pytestmark = pytest.mark.gpu
 
 
 # ------------------------------------------------------------------------------------------------
-# building block: split-bf16 GEMM on tcgen05 (descriptors, TMA, TMEM plumbing)
+# building block: split-bf16 GEMM on wgmma (descriptors, TMA, mbarrier plumbing)
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("impl", ["tc", "tc1"])
 @pytest.mark.parametrize("E", [128, 1000, 128 * 150 + 17, 128 * 301])

@@ -51,6 +51,13 @@ def mis_model(weights, impl="tc", **kw):
   return m
 
 
+def prob_rel(out, ref):
+  """Largest relative error of the softmax probabilities of `out` against those of `ref` (last axis)."""
+  p = torch.softmax(torch.as_tensor(out), -1).numpy()
+  pr = torch.softmax(torch.as_tensor(ref), -1).numpy()
+  return float(np.abs(p / pr - 1).max())
+
+
 def cu(a, dtype=None):
   t = torch.from_numpy(np.ascontiguousarray(a))
   if dtype is not None:

@@ -16,12 +16,6 @@ pytestmark = pytest.mark.gpu
 TOL = 1e-4
 
 
-def _prob_rel(out, ref):
-  p = torch.softmax(torch.as_tensor(out), -1).numpy()
-  pr = torch.softmax(torch.as_tensor(ref), -1).numpy()
-  return float(np.abs(p / pr - 1).max())
-
-
 # ------------------------------------------------------------------------------------------------
 # configs[1], the headline workload: TSP-500 k=50, batch 16 in one block-diagonal call (E = 400 000)
 # ------------------------------------------------------------------------------------------------
@@ -33,7 +27,7 @@ def test_config2_tsp500_batch16_forward_vs_oracle(weights2):
   ref = orc.encoder_forward_sparse_tsp(orc.Weights(weights2), pts, xt, np.array([969.0]), ei).numpy()
   enc = G.encoder(weights2, 2, impl="tc")
   out = enc(G.cu(pts), torch.tensor([969.0]), G.cu(xt), G.cu(ei)).cpu().numpy()
-  assert rel_linf(out, ref) < TOL and _prob_rel(out, ref) < TOL, (rel_linf(out, ref), _prob_rel(out, ref))
+  assert rel_linf(out, ref) < TOL and G.prob_rel(out, ref) < TOL, (rel_linf(out, ref), G.prob_rel(out, ref))
 
 
 def test_config2_tsp500_teacher_forced_50_steps(weights2):
@@ -203,7 +197,7 @@ def test_config4_mis_batch4_vs_oracle(weights2):
   ref = orc.encoder_forward_mis(orc.Weights(weights2), xt, np.array([905.0]), ei).numpy()
   enc = G.encoder(weights2, 2, node_only=True, impl="tc")
   out = enc(G.cu(xt), torch.tensor([905.0]), edge_index=G.cu(ei)).cpu().numpy()
-  assert rel_linf(out, ref) < TOL and _prob_rel(out, ref) < TOL, (rel_linf(out, ref), _prob_rel(out, ref))
+  assert rel_linf(out, ref) < TOL and G.prob_rel(out, ref) < TOL, (rel_linf(out, ref), G.prob_rel(out, ref))
 
 
 # ------------------------------------------------------------------------------------------------

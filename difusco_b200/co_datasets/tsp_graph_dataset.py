@@ -6,8 +6,13 @@ Same constructor, `get_example`, `__len__` and `__getitem__` item layout:
   sparse (sparse_factor  > 0): (idx[1], GraphData(x (N,2) f32, edge_index (2,N*K) i64, edge_attr (N*K,1) bool),
                                 point_indicator[1], edge_indicator[1], tour)                           :52-81
 The k-NN graph (KDTree(leaf_size=30, euclidean).query in float64, :56-57) is built by the CUDA kernel behind
-`dfb_knn_graph` (brute force in fp64, neighbours ascending with self first: identical indices).  Without a GPU the
-dataset raises - there is no CPU fallback in the product; the CPU oracle is sklearn's KDTree itself (tests).
+`dfb_knn_graph` (brute force in fp64, neighbours ascending with self first, exact ties to the smaller index).  Where
+no two of a row's first K + 1 neighbours tie exactly, that order is the only one and KDTree returns it too.  KDTree
+breaks exact ties (integer or rounded coordinates: grids, repeated points) in the order its tree traversal meets
+them, and a tie across rank K changes which neighbours are in the row.  So the kernel ranks K + 1 neighbours, the
+host recomputes their squared distances with the same expression, and only the rows with an exact tie are queried
+again with the reference's own KDTree (its queries are independent per point).  Without a GPU the dataset raises:
+the kernel builds every row, the KDTree query only resolves ties.
 """
 import numpy as np
 import torch
@@ -33,12 +38,41 @@ def knn_edge_index_gpu(points64, k, device=None, node_offset=0):
   dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
   if isinstance(points64, torch.Tensor):
     pts = points64.to(device=dev, dtype=torch.float64).contiguous()
+    host = pts.cpu().numpy()
   else:
-    pts = torch.from_numpy(np.ascontiguousarray(points64, dtype=np.float64)).to(dev)
-  n = pts.shape[0]
-  out = torch.empty((2, n * k), dtype=torch.int64, device=dev)
+    host = np.ascontiguousarray(points64, dtype=np.float64)
+    pts = None
+  if host.ndim != 2 or host.shape[1] != 2:
+    raise ValueError(f"points must be (N, 2), got {tuple(host.shape)}")
+  if not np.isfinite(host).all():
+    raise ValueError("k-NN graph: points must be finite (the reference's KDTree rejects NaN and inf)")
+  if pts is None:
+    pts = torch.from_numpy(host).to(dev)
+  n = host.shape[0]
+  kq = min(k + 1, n) if 0 < k <= n else k          # one rank beyond k shows a tie across the row's last place
+  ranked = torch.empty((2, n * kq), dtype=torch.int64, device=dev)
   _engine(dev.index if dev.index is not None else torch.cuda.current_device()).knn_graph(
-      pts.data_ptr(), n, k, node_offset, out.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+      pts.data_ptr(), n, kq, node_offset, ranked.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+  cols = ranked[1].view(n, kq)
+  nbr = cols.cpu().numpy() - node_offset
+  x, y = np.ascontiguousarray(host[:, 0]), np.ascontiguousarray(host[:, 1])
+  with np.errstate(over="ignore"):                 # the kernel's expression: float64 (x_j - x_q)^2 + (y_j - y_q)^2
+    d2 = np.take(x, nbr)
+    d2 -= x[:, None]
+    d2 *= d2
+    dy = np.take(y, nbr)
+    dy -= y[:, None]
+    dy *= dy
+    d2 += dy
+  # distances that overflow to +inf are no order KDTree can reproduce either: those rows keep the kernel's
+  tied = np.flatnonzero(((d2[:, 1:] == d2[:, :-1]) & (d2[:, 1:] < np.inf)).any(axis=1))
+  out = torch.empty((2, n * k), dtype=torch.int64, device=dev)
+  out[0] = ranked[0].view(n, kq)[:, :k].reshape(-1)
+  out[1] = cols[:, :k].reshape(-1)
+  if len(tied):
+    from sklearn.neighbors import KDTree
+    _, idx = KDTree(host, leaf_size=30, metric="euclidean").query(host[tied], k=k, return_distance=True)
+    out[1].view(n, k)[torch.from_numpy(tied).to(dev)] = torch.from_numpy(idx.astype(np.int64) + node_offset).to(dev)
   return out
 
 

@@ -1041,11 +1041,14 @@ extern "C" int dfb_knn_graph(dfb_ctx* ctx, const double* points, int64_t num_nod
   cudaStream_t st = (cudaStream_t)stream_;
   CK(ctx, cudaSetDevice(ctx->device));
   if (num_nodes < 1 || k < 1 || k > num_nodes) FAIL(ctx, DFB_E_INVALID, "bad kNN size N=%lld K=%d", (long long)num_nodes, k);
-  const size_t smem = (size_t)num_nodes * sizeof(double);
-  if (smem > 200 * 1024) FAIL(ctx, DFB_E_UNSUPPORTED, "kNN graph: N=%lld exceeds the shared-memory brute-force limit (25600)", (long long)num_nodes);
+  if ((size_t)num_nodes * sizeof(double) > 200 * 1024) FAIL(ctx, DFB_E_UNSUPPORTED, "kNN graph: N=%lld exceeds the shared-memory brute-force limit (25600)", (long long)num_nodes);
+  const size_t smem = (size_t)num_nodes * sizeof(double) + (size_t)(num_nodes + 31) / 32 * sizeof(unsigned);   // keys + taken mask
   if (!is_device_ptr(edge_index)) FAIL(ctx, DFB_E_INVALID, "edge_index must be a device pointer");
   const double* dp = points;
   if (!is_device_ptr(points)) {
+    // KDTree rejects NaN and inf; device-resident points are the caller's to check (knn_edge_index_gpu does)
+    for (int64_t i = 0; i < 2 * num_nodes; ++i)
+      if (!std::isfinite(points[i])) FAIL(ctx, DFB_E_INVALID, "kNN graph: non-finite coordinate of node %lld", (long long)(i / 2));
     ENS(ctx, ctx->d_points, (size_t)num_nodes * 2 * sizeof(double));
     CK(ctx, cudaMemcpyAsync(ctx->d_points.p, points, (size_t)num_nodes * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
     dp = (const double*)ctx->d_points.p;
@@ -1080,8 +1083,17 @@ extern "C" int dfb_two_opt(dfb_ctx* ctx, const double* points, int64_t n, int64_
   if (!points || !tours || !iterations_out) FAIL(ctx, DFB_E_INVALID, "two_opt: null argument");
   if (n < 3 || n > 46340 || batch < 1 || batch > 65535) FAIL(ctx, DFB_E_INVALID, "two_opt: bad size n=%lld batch=%lld (n in [3, 46340], batch in [1, 65535])", (long long)n, (long long)batch);
   const int N = (int)n, B = (int)batch;
-  for (int64_t k = 0; k < batch * (n + 1); ++k)
+  bool finite = true;
+  for (int64_t k = 0; k < batch * (n + 1); ++k) {
     if (tours[k] < 0 || tours[k] >= n) FAIL(ctx, DFB_E_INVALID, "two_opt: tour entry %lld out of range", (long long)tours[k]);
+    finite = finite && std::isfinite(points[2 * tours[k]]) && std::isfinite(points[2 * tours[k] + 1]);
+  }
+  if (!finite) {
+    // A NaN or inf point on a tour makes some move's change NaN; the reference's torch.min propagates it, its
+    // `min_change < -1e-6` test fails and it returns the tours unchanged after 0 iterations.
+    *iterations_out = 0;
+    return DFB_OK;
+  }
   const int T = (N + TWOOPT_TILE - 1) / TWOOPT_TILE;
   std::vector<int2> tiles;
   for (int a = 0; a < T; ++a)

@@ -372,6 +372,41 @@ def gen_tsp_decode():
   save("tsp_decode", **out)
 
 
+TWO_OPT_TIE_CAPS = (1, 7, 1000)
+
+
+class IeeeSqrt(object):
+  """Replace torch.sqrt by numpy's correctly rounded square root.  The reference runs 2-opt on the model's CUDA
+  device (pl_tsp_model.py:229-231), where torch.sqrt of float64 is correctly rounded; torch's vectorised CPU sqrt is
+  not (it is off by one ulp on some inputs), and on integer coordinates that decides which of two tied moves wins."""
+
+  def __enter__(self):
+    self.orig = torch.sqrt
+    torch.sqrt = lambda x: torch.from_numpy(np.sqrt(x.numpy()))
+    return self
+
+  def __exit__(self, *a):
+    torch.sqrt = self.orig
+
+
+def gen_two_opt_ties():
+  """batched_two_opt_torch of the reference (CPU device, IEEE sqrt) on instances whose moves tie exactly: three random
+  tours per instance, run as one batch of 3 and as the first tour alone, at every cap of TWO_OPT_TIE_CAPS."""
+  from oracle import tsp_decode_oracle as orc
+  tu = _reference_tsp_utils()
+  out = {}
+  for s, (name, pts) in enumerate(sorted(orc.tie_instances().items())):
+    tours = orc.random_tours(len(pts), 3, seed=100 + s)
+    out[f"{name}/points"], out[f"{name}/tours"] = pts, tours
+    for b in (1, 3):
+      for cap in TWO_OPT_TIE_CAPS:
+        with IeeeSqrt():
+          solved, ns = tu.batched_two_opt_torch(pts, tours[:b], max_iterations=cap, device="cpu")
+        out[f"{name}/b{b}_cap{cap}"], out[f"{name}/b{b}_cap{cap}_iters"] = solved, np.int64(ns)
+    print(name, len(pts), [int(out[f"{name}/b{b}_cap1000_iters"]) for b in (1, 3)])
+  save("two_opt_ties", **out)
+
+
 def gen_mcts_txt():
   """tsp_mcts/convert_numpy_to_txt.py of the reference, run unmodified on small dense heat maps.  The script needs
   `fire` (absent: stubbed, main() is called directly) and np.bool (removed in numpy >= 1.24: aliased here only)."""
@@ -434,6 +469,8 @@ if __name__ == "__main__":
     gen_mis_decode()
   if a.only in ("", "tsp_decode"):
     gen_tsp_decode()
+  if a.only in ("", "two_opt_ties"):
+    gen_two_opt_ties()
   if a.only in ("", "mcts_txt"):
     gen_mcts_txt()
   if a.only in ("", "ref_copy"):

@@ -125,6 +125,19 @@ def test_two_opt_oracle_matches_reference(name, k, par):
     assert np.array_equal(solved, g[f"{name}/two_opt_{cap}"]) and ns == int(g[f"{name}/two_opt_{cap}_iters"])
 
 
+@pytest.mark.parametrize("name", sorted(orc.tie_instances()))
+def test_two_opt_oracle_matches_reference_on_ties(name):
+  """tests/golden/two_opt_ties.npz: the reference's 2-opt on instances whose moves tie exactly (first occurrence wins),
+  as one batch of three tours and as the first tour alone.  The fixture's points are the generator's."""
+  g = _load_golden("two_opt_ties")
+  pts = g[f"{name}/points"]
+  assert np.array_equal(pts, orc.tie_instances()[name])
+  for b in (1, 3):
+    for cap in (1, 7, 1000):
+      solved, ns = orc.two_opt(pts, g[f"{name}/tours"][:b], cap)
+      assert ns == int(g[f"{name}/b{b}_cap{cap}_iters"]) and np.array_equal(solved, g[f"{name}/b{b}_cap{cap}"])
+
+
 def test_two_opt_requires_cuda_device():
   with pytest.raises(RuntimeError):
     tu.batched_two_opt_torch(np.zeros((4, 2)), np.array([[0, 1, 2, 3, 0]]), device="cpu")

@@ -20,7 +20,7 @@ SYMBOLS = [
     "dfb_encoder_forward", "dfb_denoise_step", "dfb_denoise", "dfb_denoise_host",
     "dfb_launch_count", "dfb_profile_begin", "dfb_profile_end", "dfb_debug_edge_gemm",
     "dfb_debug_phase_cycles", "dfb_debug_watchdog", "dfb_knn_graph", "dfb_set_graph_capture",
-    "dfb_tsp_merge_sparse", "dfb_tsp_merge_order", "dfb_two_opt", "dfb_write_heatmap_txt",
+    "dfb_set_phase_timing", "dfb_tsp_merge_sparse", "dfb_tsp_merge_order", "dfb_two_opt", "dfb_write_heatmap_txt",
 ]
 
 _lib = None
@@ -61,6 +61,7 @@ def lib():
   L.dfb_debug_phase_cycles.argtypes = [vp, C.POINTER(C.c_uint64)]
   L.dfb_debug_watchdog.argtypes = [vp, C.POINTER(C.c_int)]
   L.dfb_set_graph_capture.argtypes = [vp, i32]
+  L.dfb_set_phase_timing.argtypes = [vp, i32]
   L.dfb_knn_graph.argtypes = [vp, vp, i64, i32, i64, vp, vp]
   L.dfb_tsp_merge_sparse.argtypes = [vp, i64, vp, vp, i64, i32, vp, C.POINTER(i64)]
   L.dfb_tsp_merge_order.argtypes = [i64, vp, i64, vp, C.POINTER(i64)]
@@ -266,7 +267,13 @@ class Context(object):
     lib().dfb_debug_watchdog(self._h, out)
     return [int(x) for x in out]
 
+  def set_phase_timing(self, enabled):
+    """Route the product edge-layer launches to the kernel with phase timers (read them with debug_phase_cycles)."""
+    self._ck(lib().dfb_set_phase_timing(self._h, int(bool(enabled))))
+
   def debug_phase_cycles(self):
+    """Read and reset the 32 phase counters: [tiles, total, convert, gemm1 wait, gemm1 mma, e1, reduce, ln, gemm2 wait,
+    gemm2 mma, e4, 0...] (cycles summed over consumer warpgroups; see include/difusco_b200.h)."""
     out = (C.c_uint64 * 32)()
     self._ck(lib().dfb_debug_phase_cycles(self._h, out))
     return [int(x) for x in out]

@@ -72,10 +72,11 @@ struct dfb_ctx {
   struct LoopKey {
     uint64_t buf_gen = ~0ull;
     int steps = 0, diffusion = 0, impl = 0, agg = 0;
+    bool timed = false;
     const void* uniforms = nullptr;
     bool operator==(const LoopKey& o) const {
       return buf_gen == o.buf_gen && steps == o.steps && diffusion == o.diffusion && impl == o.impl && agg == o.agg &&
-             uniforms == o.uniforms;
+             timed == o.timed && uniforms == o.uniforms;
     }
   } loop_key;
   int64_t loop_launches = 0;     // kernel launches inside one replay of the captured loop
@@ -893,7 +894,7 @@ extern "C" int dfb_denoise(dfb_ctx* ctx, int diffusion_type, float* xt, int step
   if (want_graph) {
     dfb_ctx::LoopKey key;
     key.buf_gen = ctx->buf_gen; key.steps = steps; key.diffusion = diffusion_type; key.impl = ctx->edge_impl;
-    key.agg = ctx->agg_mode; key.uniforms = uniforms;
+    key.agg = ctx->agg_mode; key.timed = ctx->tc.timed; key.uniforms = uniforms;
     if (!ctx->loop_exec || !(ctx->loop_key == key)) {
       if (ctx->loop_exec) {
         cudaGraphExecDestroy(ctx->loop_exec);
@@ -940,6 +941,12 @@ extern "C" int dfb_set_graph_capture(dfb_ctx* ctx, int enabled) {
   if (!ctx) return DFB_E_INVALID;
   ctx->capture_enabled = enabled != 0;
   ctx->capture_broken = false;
+  return DFB_OK;
+}
+
+extern "C" int dfb_set_phase_timing(dfb_ctx* ctx, int enabled) {
+  if (!ctx) return DFB_E_INVALID;
+  ctx->tc.timed = enabled != 0;   // part of the captured loop's key: the next dfb_denoise re-captures
   return DFB_OK;
 }
 
@@ -1010,8 +1017,8 @@ extern "C" int dfb_debug_edge_gemm(dfb_ctx* ctx, int layer, const float* e_in, f
   return DFB_OK;
 }
 
-// Test/tuning hook: read and reset the per-phase cycle counters of the edge kernel.  The wgmma kernels record
-// none, so the counters read back as zero.  out[32] host.
+// Test/tuning hook: read and reset the per-phase cycle counters of the edge kernel (slots PH_* of edge_layer_tc.cuh).
+// Only the timed product kernel (dfb_set_phase_timing) records them; otherwise they read back as zero.  out[32] host.
 extern "C" int dfb_debug_phase_cycles(dfb_ctx* ctx, unsigned long long* out) {
   if (!ctx || !out) return DFB_E_INVALID;
   CK(ctx, cudaSetDevice(ctx->device));

@@ -39,6 +39,10 @@ constexpr int TC_KCH = 64;                      // K elements per chunk = one 12
 constexpr int TC_B_BYTES = 256 * 128;           // one weight chunk [256 rows x 64 K] bf16 (hi or lo)
 constexpr int TC_A_CHUNK = WG_ROWS * 128;       // one operand chunk [64 rows x 64 K] bf16 (hi or lo)
 constexpr int TC_A_BYTES = 8 * TC_A_CHUNK;      // 4 K-chunks x (hi, lo) per warpgroup = 64 KB = [64][256] fp32 messages
+// Loads a consumer thread issues before it uses the first of them (memory-level parallelism of the epilogues), sized
+// so that they fit next to the 128 accumulator registers without spills:
+constexpr int CONV_BATCH = 16;   // conversion: float4 row loads of 32
+constexpr int E4_BATCH = 16;     // E4: float2 e_in loads of a row half of 32
 
 template <int NWG>
 struct TcCfg {
@@ -76,6 +80,7 @@ struct TcParams {
   int lin_nb;             // 256-column output blocks per row tile: 4 (U|V|A|B) or 1 (embedding linears)
   int lin_w_row;          // first weight row of block 0 in the bf16 arena (blocks are 512 rows apart: hi, lo)
   int* error_flag;
+  unsigned long long* phase_cycles;   // [32] phase timers (k_edge_layer_wg2_timed only), see PH_*
   int write_e, e_zero, agg_mode;
   int w_row_base;         // row of this layer's C_hi block in the bf16 weight arena tensor map
   int n_tiles;
@@ -134,7 +139,8 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // Keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma window.
 __device__ __forceinline__ void acc_fence(float (&d)[128]) {
 #pragma unroll
@@ -207,13 +213,32 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
+// Phase timers of the instrumented entry point k_edge_layer_wg2_timed: slots of TcParams::phase_cycles, summed over
+// every consumer warpgroup of the launch (SM clock cycles read by thread 0 of the warpgroup).  The phases partition the
+// tile loop, so their sum never exceeds PH_TOTAL.
+enum {
+  PH_TILES = 0,   // tiles processed (one count per warpgroup and tile)
+  PH_TOTAL,       // cycles from the first tile to the end of the tile loop
+  PH_CONVERT,     // row table + fp32 -> bf16 hi/lo conversion of GEMM1's A operand
+  PH_G1_WAIT,     // GEMM1: waits for weight chunks (full barriers)
+  PH_G1_MMA,      // GEMM1: wgmma issue and drain
+  PH_E1,          // gathers, gate, messages to shared memory
+  PH_REDUCE,      // message reduction into partials
+  PH_LN,          // both LayerNorms, SiLU, GEMM2 A operand
+  PH_G2_WAIT,     // GEMM2: waits for weight chunks
+  PH_G2_MMA,      // GEMM2: wgmma issue and drain
+  PH_E4,          // residual update of the edge stream
+  PH_COUNT
+};
+
 // ----------------------------------------------------------------------------------------------
 // Accumulator fragment of wgmma m64n256 (per thread: warp wi of the warpgroup, lane = 4 * g + t):
 //   acc[4 j + 2 h + b]  ->  row 16 wi + g + 8 h,  column 8 j + 2 t + b        (j < 32, h, b in {0, 1})
 // so the 256 columns of a row are spread over the 4 threads of a quad: row reductions are 64 thread-local terms
 // plus two shuffles.
 // ----------------------------------------------------------------------------------------------
-template <int NWG>
+// TIMED adds the phase timers (clock reads pin instruction order, so the product entry points are built without).
+template <int NWG, bool TIMED = false>
 __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, const TcParams& P) {
   using Cfg = TcCfg<NWG>;
   constexpr int NSTAGE = Cfg::NSTAGE;
@@ -283,14 +308,39 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
   uint32_t u = 0;
   float acc[128];
 
-  // 8 weight chunks (4 K-chunks x hi, lo) against this warpgroup's A operand (hi, lo at chunk 2 kc, 2 kc + 1)
-  auto gemm = [&]() {
+  // phase timers (TIMED only): thread 0 of the warpgroup adds each phase's cycles straight into P.phase_cycles (fire-
+  // and-forget reductions), so the timers keep two 32-bit clock readings in registers (differences of the low clock
+  // word stay exact for spans below 2^32 cycles, ~2 s)
+  uint32_t t_mark = 0, t_start = 0;
+  if constexpr (TIMED) t_start = t_mark = (uint32_t)clock();
+  auto record = [&](int slot, uint32_t v) {
+    if constexpr (TIMED) {
+      if (tid == 0) atomicAdd(P.phase_cycles + slot, (unsigned long long)v);
+    }
+  };
+  auto mark = [&](int slot) {
+    if constexpr (TIMED) {
+      const uint32_t now = (uint32_t)clock();
+      record(slot, now - t_mark);
+      t_mark = now;
+    }
+  };
+
+  // 8 weight chunks (4 K-chunks x hi, lo) against this warpgroup's A operand (hi, lo at chunk 2 kc, 2 kc + 1).
+  // One wgmma group stays in flight across chunk boundaries: chunk i is issued before chunk i - 1's stage is released,
+  // so the wait for chunk i + 1's weights overlaps chunk i's tensor work.  The wgmmas still run in issue order on acc.
+  auto gemm = [&](int wait_slot, int mma_slot) {
+    uint32_t waited = 0;
     acc_fence(acc);
     wgmma_fence();
+    int s_prev = 0;
 #pragma unroll
     for (int i = 0; i < 8; ++i, ++u) {
       const int s = u % NSTAGE;
+      uint32_t w0 = 0;
+      if constexpr (TIMED) w0 = (uint32_t)clock();
       mbar_wait(&full[s], (u / NSTAGE) & 1, P.error_flag, 2);
+      if constexpr (TIMED) waited += (uint32_t)clock() - w0;
       const uint32_t b = smem_base + Cfg::OFF_B + s * TC_B_BYTES;
       const uint32_t ahi = a_base + (i >> 1) * 2 * TC_A_CHUNK, alo = ahi + TC_A_CHUNK;
 #pragma unroll
@@ -300,14 +350,27 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
         if ((i & 1) == 0) wgmma_bf16(acc, wgmma_desc_sw128(alo + ks * 32), db, 1u);   // lo*hi
       }
       wgmma_commit();
-      wgmma_wait_all();
-      acc_fence(acc);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty[s]);
+      if (i > 0) {
+        wgmma_wait<1>();   // chunk i - 1 has been read
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s_prev]);
+      }
+      s_prev = s;
+    }
+    wgmma_wait<0>();
+    acc_fence(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s_prev]);
+    if constexpr (TIMED) {
+      const uint32_t now = (uint32_t)clock();
+      record(wait_slot, waited);
+      record(mma_slot, now - t_mark - waited);
+      t_mark = now;
     }
   };
 
   for (int tile = blockIdx.x; tile < P.n_tiles; tile += gridDim.x) {
+    record(PH_TILES, 1);
     const int row_tile = (lin && P.lin_nb == 4) ? (tile >> 2) : tile;
     const int s_base = row_tile * Cfg::TILE + wg * WG_ROWS;   // first edge (input row) of this warpgroup
     if (tid < WG_ROWS) {
@@ -328,20 +391,30 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
     wg_bar();   // row table visible; every warp has left the previous tile's GEMM2 (A operand area free)
 
     // ---------------- GEMM1 A operand: fp32 rows -> bf16 hi/lo, K-major 128B-swizzled chunks ----------------
-#pragma unroll 4
-    for (int it = 0; it < 32; ++it) {
-      const int item = it * 128 + tid;
-      const int rr = item >> 6, k4 = item & 63;
-      const float4 x = __ldcg(reinterpret_cast<const float4*>(w_src[rr]) + k4);
-      uint2 hi, lo;
-      split4(x, hi, lo);
-      const uint32_t off = (k4 >> 4) * 2 * TC_A_CHUNK + sw128_off(rr, (k4 & 15) >> 1) + (k4 & 1) * 8;
-      *reinterpret_cast<uint2*>(a_reg + off) = hi;
-      *reinterpret_cast<uint2*>(a_reg + off + TC_A_CHUNK) = lo;
+    // CONV_BATCH row loads of a thread are issued before the first split: one memory round trip per batch.
+#pragma unroll
+    for (int it0 = 0; it0 < 32; it0 += CONV_BATCH) {
+      float4 x[CONV_BATCH];
+#pragma unroll
+      for (int q = 0; q < CONV_BATCH; ++q) {
+        const int item = (it0 + q) * 128 + tid;
+        x[q] = __ldcg(reinterpret_cast<const float4*>(w_src[item >> 6]) + (item & 63));
+      }
+#pragma unroll
+      for (int q = 0; q < CONV_BATCH; ++q) {
+        const int item = (it0 + q) * 128 + tid;
+        const int rr = item >> 6, k4 = item & 63;
+        uint2 hi, lo;
+        split4(x[q], hi, lo);
+        const uint32_t off = (k4 >> 4) * 2 * TC_A_CHUNK + sw128_off(rr, (k4 & 15) >> 1) + (k4 & 1) * 8;
+        *reinterpret_cast<uint2*>(a_reg + off) = hi;
+        *reinterpret_cast<uint2*>(a_reg + off + TC_A_CHUNK) = lo;
+      }
     }
     fence_proxy_async();   // generic-proxy stores -> visible to wgmma
     wg_bar();
-    gemm();
+    mark(PH_CONVERT);
+    gemm(PH_G1_WAIT, PH_G1_MMA);
 
     const int sa = s_base + lr0, sb = sa + 8;
     const bool va = sa < n_rows, vb = sb < n_rows;
@@ -396,6 +469,7 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
       }
     }
     wg_bar();   // messages of all 64 rows are in shared memory
+    mark(PH_E1);
     // row-segment reduction: thread = column, rows of each 32-edge group in order (the fp32 kernel's order)
 #pragma unroll 1
     for (int g2 = 0; g2 < WG_ROWS / GROUP; ++g2) {
@@ -423,6 +497,7 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
       }
     }
     wg_bar();   // messages consumed: the area takes GEMM2's A operand next; the row table may be rewritten
+    mark(PH_REDUCE);
     if (!P.write_e) continue;   // MIS last layer: the edge stream is never read again (gnn_encoder.py:412)
 
     // ---------------- E2 / E3: e_til = relu(LN_e(e_hat)) + tau;  s = silu(LN_O(e_til)) -> GEMM2 A operand ----------------
@@ -477,7 +552,8 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
     }
     fence_proxy_async();
     wg_bar();
-    gemm();   // GEMM2: acc = s * O^T
+    mark(PH_LN);
+    gemm(PH_G2_WAIT, PH_G2_MMA);   // GEMM2: acc = s * O^T
 
     // ---------------- E4: e = e_in + O(s) + b_O (in place) ----------------
 #pragma unroll
@@ -485,16 +561,25 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
       if (!(h ? vb : va)) continue;
       const float* src = h ? src_b : src_a;
       float* dst = P.e + (size_t)(h ? sb : sa) * H;
+      // the row is updated in place: its e_in values are loaded in batches before any of them is overwritten (the
+      // compiler cannot move a load above a store to the same row by itself)
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int c = 8 * j + 2 * t4;
-        const float2 ein = __ldcg(reinterpret_cast<const float2*>(src + c));
-        const float2 bo = *reinterpret_cast<const float2*>(prm + 5 * H + c);
-        __stcg(reinterpret_cast<float2*>(dst + c),
-               make_float2((ein.x + acc[4 * j + 2 * h]) + bo.x, (ein.y + acc[4 * j + 2 * h + 1]) + bo.y));
+      for (int j0 = 0; j0 < 32; j0 += E4_BATCH) {
+        float2 ein[E4_BATCH];
+#pragma unroll
+        for (int q = 0; q < E4_BATCH; ++q) ein[q] = __ldcg(reinterpret_cast<const float2*>(src + 8 * (j0 + q) + 2 * t4));
+#pragma unroll
+        for (int q = 0; q < E4_BATCH; ++q) {
+          const int j = j0 + q, c = 8 * j + 2 * t4;
+          const float2 bo = *reinterpret_cast<const float2*>(prm + 5 * H + c);
+          __stcg(reinterpret_cast<float2*>(dst + c),
+                 make_float2((ein[q].x + acc[4 * j + 2 * h]) + bo.x, (ein[q].y + acc[4 * j + 2 * h + 1]) + bo.y));
+        }
       }
     }
+    mark(PH_E4);
   }
+  if constexpr (TIMED) record(PH_TOTAL, (uint32_t)clock() - t_start);
 }
 
 // Kernel entry points.  The two-warpgroup kernel (128-row tiles) is the product path; the one-warpgroup kernel
@@ -502,6 +587,11 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
 __global__ void __launch_bounds__(TcCfg<2>::THREADS, 1)
 k_edge_layer_wg2(const __grid_constant__ CUtensorMap wmap, const TcParams P) {
   edge_layer_wg_body<2>(wmap, P);
+}
+// the product kernel with phase timers (dfb_set_phase_timing): same results, read back by dfb_debug_phase_cycles
+__global__ void __launch_bounds__(TcCfg<2>::THREADS, 1)
+k_edge_layer_wg2_timed(const __grid_constant__ CUtensorMap wmap, const TcParams P) {
+  edge_layer_wg_body<2, true>(wmap, P);
 }
 __global__ void __launch_bounds__(TcCfg<1>::THREADS, 1)
 k_edge_layer_wg1(const __grid_constant__ CUtensorMap wmap, const TcParams P) {
@@ -531,7 +621,8 @@ struct TcState {
   float* lin_out = nullptr;
   const float* lin_bias = nullptr;
   int lin_rows = 0, lin_nb = 4, lin_w_row = 0;
-  unsigned long long* phase_cycles = nullptr;   // dfb_debug_phase_cycles: these kernels record none (stays zero)
+  unsigned long long* phase_cycles = nullptr;   // [32] dfb_debug_phase_cycles; only the timed kernel adds to it
+  bool timed = false;                           // product launches go to k_edge_layer_wg2_timed
 };
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -541,6 +632,8 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
 inline int tc_init(TcState* st, int num_sms) {
   st->num_sms = num_sms;
   cudaError_t e = cudaFuncSetAttribute(k_edge_layer_wg2, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<2>::SMEM_ALLOC);
+  if (e == cudaSuccess)
+    e = cudaFuncSetAttribute(k_edge_layer_wg2_timed, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<2>::SMEM_ALLOC);
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute(k_edge_layer_wg1, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<1>::SMEM_ALLOC);
   if (e == cudaSuccess)
@@ -612,6 +705,7 @@ inline int tc_launch_edge_layer(TcState* st, int l, float* e, const float* uvab,
   P.e = e; P.uvab = uvab; P.partials = partials; P.g = g; P.lp = lp; P.tvec = tvec_edge;
   P.xt_lut = xt_lut; P.lut = lut; P.zero_row = st->zero_row; P.debug_acc = st->debug_acc;
   P.error_flag = st->error_flag;
+  P.phase_cycles = st->phase_cycles;
   P.write_e = (st->debug_acc || st->lin_out) ? 0 : write_e;
   P.e_zero = e_zero; P.agg_mode = agg_mode;
   P.w_row_base = l * 12 * H;
@@ -621,6 +715,8 @@ inline int tc_launch_edge_layer(TcState* st, int l, float* e, const float* uvab,
   const int grid = P.n_tiles < st->num_sms ? P.n_tiles : st->num_sms;
   if (st->lin_out) k_linear_wg2<<<grid, TcCfg<2>::THREADS, TcCfg<2>::SMEM_ALLOC, stream>>>(st->wmap, P);
   else if (nwg == 1) k_edge_layer_wg1<<<grid, TcCfg<1>::THREADS, TcCfg<1>::SMEM_ALLOC, stream>>>(st->wmap, P);
+  else if (st->timed && !st->debug_acc)
+    k_edge_layer_wg2_timed<<<grid, TcCfg<2>::THREADS, TcCfg<2>::SMEM_ALLOC, stream>>>(st->wmap, P);
   else k_edge_layer_wg2<<<grid, TcCfg<2>::THREADS, TcCfg<2>::SMEM_ALLOC, stream>>>(st->wmap, P);
   cudaError_t err = cudaGetLastError();
   if (err != cudaSuccess) {

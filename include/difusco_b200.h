@@ -176,9 +176,17 @@ int dfb_profile_end(dfb_ctx* ctx, double* edge_kernel_ms, int64_t* edge_kernel_l
  * acc_out (E,256).  DEVICE pointers.  Used by the parity tests to localise failures. */
 int dfb_debug_edge_gemm(dfb_ctx* ctx, int layer, const float* e_in, float* acc_out, void* stream);
 
-/* Tuning hook: per-phase cycle counters of the edge kernels; out must hold 32 unsigned 64-bit values (host).  The wgmma
- * kernels record none: the values read back as zero.  Read-and-reset. */
+/* Tuning hook: per-phase cycle counters of the edge kernel; out must hold 32 unsigned 64-bit values (host).  Only the
+ * timed product kernel records them (dfb_set_phase_timing); otherwise the values read back as zero.  Read-and-reset.
+ * Slots, each summed over every consumer warpgroup of every launch (SM clock cycles):
+ *   0 tiles, 1 total cycles of the tile loop, 2 row table + conversion, 3 GEMM1 weight waits, 4 GEMM1 wgmma issue and
+ *   drain, 5 gathers + gate + messages, 6 message reduction, 7 LayerNorms + SiLU, 8 GEMM2 weight waits, 9 GEMM2 wgmma
+ *   issue and drain, 10 residual update.  Slots 2..10 partition the tile loop, so their sum is at most slot 1. */
 int dfb_debug_phase_cycles(dfb_ctx* ctx, unsigned long long* out);
+
+/* Tuning hook: enabled != 0 routes the product edge-layer launches to a copy of the kernel with phase timers (same
+ * results; the timer reads cost a little time).  Changing it re-captures the dfb_denoise loop. */
+int dfb_set_phase_timing(dfb_ctx* ctx, int enabled);
 
 /* Diagnostic: watchdog record of the tensor-core kernel's bounded barrier waits (host-mapped memory, readable after a
  * launch failure): out[4] = {wait-site code or 0, blockIdx.x, parity, threadIdx.x}. */

@@ -754,7 +754,8 @@ static int run_forward(dfb_ctx* ctx, const float* xt, const float* tvec, bool bi
   const int bps = (rps + GN_ROWS_PER_BLOCK - 1) / GN_ROWS_PER_BLOCK;
   k_gn_partial<<<dim3(bps, ctx->gn_segments), 256, 0, st>>>(Z, rps, (double*)ctx->gn_part.p);
   CKL(ctx);
-  k_gn_final<<<dim3(ctx->gn_segments, 32), 256, 0, st>>>((const double*)ctx->gn_part.p, bps, rps, (float*)ctx->gn_stats.p);
+  k_gn_final<<<dim3(ctx->gn_segments, 32), 256, 0, st>>>((const double*)ctx->gn_part.p, Z, bps, rps,
+                                                      (float*)ctx->gn_stats.p);
   CKL(ctx);
   k_head<<<(R + 255) / 256, 256, 0, st>>>(Z, R, rps, (const float*)ctx->gn_stats.p, ctx->node_only ? nullptr : g.perm,
                                       ctx->hp, pa);

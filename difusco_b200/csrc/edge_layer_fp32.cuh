@@ -124,15 +124,16 @@ __global__ void __launch_bounds__(256) k_edge_layer_fp32(float* __restrict__ e, 
   }
   __syncthreads();
 
-  float bo = lp.b_O[c];
+  // b_O is added after the dot product (a large bias would otherwise round every product at its ulp)
+  const float bo = lp.b_O[c];
 #pragma unroll
-  for (int r = 0; r < EF_ROWS; ++r) acc[r] = bo;
+  for (int r = 0; r < EF_ROWS; ++r) acc[r] = 0.f;
   ef_tile_matvec(X, lp.Wt_O, c, acc);
 #pragma unroll
   for (int r = 0; r < EF_ROWS; ++r)
     if (r < nrows) {
       size_t o = (size_t)(s0 + r) * H + c;
-      e[o] = e[o] + acc[r];
+      e[o] = e[o] + (acc[r] + bo);
     }
 }
 

@@ -67,23 +67,24 @@ __global__ void __launch_bounds__(256) k_time_vectors(const float* __restrict__ 
     te[c] = (c < 128) ? cosf(a) : sinf(a);
   }
   __syncthreads();
+  // biases are added after each dot product (see k_linear)
   if (c < TE) {
-    float acc = tp.b0[c];
+    float acc = 0.0f;
     for (int k = 0; k < H; ++k) acc = fmaf(te[k], tp.Wt0[k * TE + c], acc);
-    h1[c] = fmaxf(acc, 0.0f);
+    h1[c] = fmaxf(acc + tp.b0[c], 0.0f);
   }
   __syncthreads();
   if (c < TE) {
-    float acc = tp.b2[c];
+    float acc = 0.0f;
     for (int k = 0; k < TE; ++k) acc = fmaf(h1[k], tp.Wt2[k * TE + c], acc);
-    r[c] = fmaxf(acc, 0.0f);   // every time_embed_layers[l] starts with ReLU
+    r[c] = fmaxf(acc + tp.b2[c], 0.0f);   // every time_embed_layers[l] starts with ReLU
   }
   __syncthreads();
   for (int l = 0; l < L; ++l) {
     const float* W = layers[l].Wt_tau;
-    float acc = layers[l].b_tau[c];
+    float acc = 0.0f;
     for (int k = 0; k < TE; ++k) acc = fmaf(r[k], W[k * H + c], acc);
-    tvec[((size_t)s * L + l) * H + c] = acc;
+    tvec[((size_t)s * L + l) * H + c] = acc + layers[l].b_tau[c];
   }
 }
 
@@ -106,10 +107,12 @@ __global__ void __launch_bounds__(256) k_linear(const float* __restrict__ X, con
     reinterpret_cast<float4*>(&xs[r][0])[k4] = v;
   }
   __syncthreads();
+  // the bias is added after the dot product: an accumulator started at a bias much larger than the products would
+  // round every product at the bias's ulp
   float acc[LIN_ROWS];
-  float bias = b ? b[c] : 0.0f;
+  const float bias = b ? b[c] : 0.0f;
 #pragma unroll
-  for (int r = 0; r < LIN_ROWS; ++r) acc[r] = bias;
+  for (int r = 0; r < LIN_ROWS; ++r) acc[r] = 0.0f;
   for (int k = 0; k < H; k += 4) {
     float w0 = Wt[(size_t)(k + 0) * N + c], w1 = Wt[(size_t)(k + 1) * N + c];
     float w2 = Wt[(size_t)(k + 2) * N + c], w3 = Wt[(size_t)(k + 3) * N + c];
@@ -124,7 +127,7 @@ __global__ void __launch_bounds__(256) k_linear(const float* __restrict__ X, con
   }
 #pragma unroll
   for (int r = 0; r < LIN_ROWS; ++r)
-    if (r0 + r < R) Y[(size_t)(r0 + r) * N + c] = acc[r];
+    if (r0 + r < R) Y[(size_t)(r0 + r) * N + c] = acc[r] + bias;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -192,10 +195,15 @@ __global__ void __launch_bounds__(256) k_node_update(float* __restrict__ h, cons
 // ---------------------------------------------------------------------------------------------
 // Head GroupNorm32(32, 256) statistics over ALL rows of a segment (gnn_encoder.py:400-401: the
 // batch dim is 1, so every edge of the call shares the statistics; nn.py:17-19).
-// Two passes in fp64 partials: 3.2 M values per group would lose the 1e-4 contract in fp32
-// E[x^2]-E[x]^2 form (the reference's own CPU channels-last kernel does lose it when |mean|>>std).
+// fp32 runs of <= 32 rows, combined in fp64 partials: 3.2 M values per group would lose the 1e-4 contract in fp32
+// E[x^2]-E[x]^2 form (the reference's own CPU channels-last kernel does lose it when |mean|>>std).  The runs sum
+// x - pivot, with one pivot per (segment, group): the group's first channel in the segment's first row.  Without it
+// the fp32 runs of x^2 round at |mean|^2 * 2^-24, which is the whole variance once |mean| / std reaches ~1000.
 // ---------------------------------------------------------------------------------------------
 constexpr int GN_ROWS_PER_BLOCK = 256;
+__device__ __forceinline__ float gn_pivot(const float* Z, int seg, int rows_per_seg, int group) {
+  return Z[(size_t)seg * rows_per_seg * H + group * 8];
+}
 __global__ void __launch_bounds__(256) k_gn_partial(const float* __restrict__ Z, int rows_per_seg,
                                                     double* __restrict__ part) {
   // grid (blocks_per_seg, segs).  thread = channel; fp32 run of <= 32 rows, then fp64.
@@ -203,12 +211,13 @@ __global__ void __launch_bounds__(256) k_gn_partial(const float* __restrict__ Z,
   int r0 = blockIdx.x * GN_ROWS_PER_BLOCK;
   int r1 = min(r0 + GN_ROWS_PER_BLOCK, rows_per_seg);
   const float* base = Z + ((size_t)seg * rows_per_seg) * H + c;
+  const float piv = gn_pivot(Z, seg, rows_per_seg, c >> 3);
   double S = 0.0, Q = 0.0;
   for (int r = r0; r < r1; r += 32) {
     float s = 0.f, q = 0.f;
     int re = min(r + 32, r1);
     for (int rr = r; rr < re; ++rr) {
-      float v = base[(size_t)rr * H];
+      float v = base[(size_t)rr * H] - piv;
       s += v;
       q = fmaf(v, v, q);
     }
@@ -227,7 +236,8 @@ __global__ void __launch_bounds__(256) k_gn_partial(const float* __restrict__ Z,
     part[o + 1] = Q;
   }
 }
-__global__ void __launch_bounds__(256) k_gn_final(const double* __restrict__ part, int blocks_per_seg, int rows_per_seg,
+__global__ void __launch_bounds__(256) k_gn_final(const double* __restrict__ part, const float* __restrict__ Z,
+                                                  int blocks_per_seg, int rows_per_seg,
                                                   float* __restrict__ stats /* [segs][32][2] mean, rstd */) {
   // grid (segs, 32 groups); 256 threads stride over the per-block partials, then a fixed-shape fp64 tree
   // (warp shuffles + 8 warp results in shared memory): deterministic
@@ -247,10 +257,10 @@ __global__ void __launch_bounds__(256) k_gn_final(const double* __restrict__ par
     S = 0.0; Q = 0.0;
     for (int i = 0; i < 8; ++i) { S += sh[i][0]; Q += sh[i][1]; }
     double n = (double)rows_per_seg * 8.0;
-    double mean = S / n;
-    double var = Q / n - mean * mean;
+    double dm = S / n;                       // mean - pivot
+    double var = Q / n - dm * dm;
     if (var < 0.0) var = 0.0;
-    stats[(seg * 32 + gidx) * 2] = (float)mean;
+    stats[(seg * 32 + gidx) * 2] = (float)((double)gn_pivot(Z, seg, rows_per_seg, gidx) + dm);
     stats[(seg * 32 + gidx) * 2 + 1] = (float)(1.0 / sqrt(var + (double)LN_EPS));
   }
 }

@@ -63,3 +63,89 @@ def cu(a, dtype=None):
   if dtype is not None:
     t = t.to(dtype)
   return t.cuda()
+
+
+# ------------------------------------------------------------------------------------------------
+# Weight regimes: the synthetic weights moved into value ranges a trained checkpoint reaches (confident heads, large
+# linears, an offset head GroupNorm input, extreme norm gains, the reference's zero-initialised output layers).
+# `fwd(w)` -> (logits (R, out), head input (R, 256)) is the fp64 oracle on the graph the regime is calibrated on;
+# `node_head` says the head reads h (MIS) rather than e.
+# ------------------------------------------------------------------------------------------------
+REGIMES = ["R0", "R1", "R1x", "R2", "R3", "R4_10", "R4_100", "R4_1000", "R5", "R6"]
+N_LAYERS = 12
+NORM_PREFIXES = ["out.0."] + [f"layers.{l}.norm_{s}." for l in range(N_LAYERS) for s in "he"] + \
+                [f"per_layer_out.{l}.0." for l in range(N_LAYERS)]
+
+
+def head_group_stats(z):
+  """Per-group mean and (biased) std of the head GroupNorm32 input z (R, 256), over all rows."""
+  g = np.asarray(z, np.float64).reshape(z.shape[0], 32, -1)
+  return g.mean((0, 2)), g.std((0, 2))
+
+
+def _scale_linears(w, f):
+  for l in range(N_LAYERS):
+    for n in "UVABC":
+      w[f"layers.{l}.{n}.weight"] *= f
+    w[f"per_layer_out.{l}.2.weight"] *= f
+
+
+def _offset_head_input(w, fwd, node_head, ratio):
+  """Shift each head group by a constant so that its |mean| / std is `ratio` on the calibration graph."""
+  m, s = head_group_stats(fwd(w)[1])
+  key = f"time_embed_layers.{N_LAYERS - 1}.1.bias" if node_head else f"per_layer_out.{N_LAYERS - 1}.2.bias"
+  w[key] += np.repeat(ratio * s - m, 8).astype(np.float32)
+
+
+def _confident_head(w, fwd, target):
+  """Scale out.2 so that the largest |l1 - l0| (|x0| for one channel) is `target`; two channels: also move the
+  decision point to the 90th percentile of l1 - l0, so most rows are confidently class 0, as in a trained TSP head
+  (2 of the K = 20 edges of a node are tour edges)."""
+  out = fwd(w)[0]
+  out = out.reshape(-1, out.shape[-1])
+  if out.shape[1] == 1:
+    a = target / np.abs(out).max()
+    q = 0.0
+  else:
+    d = out[:, 1] - out[:, 0]
+    q = float(np.quantile(d, 0.9))
+    a = target / np.abs(d - q).max()
+  w["out.2.weight"] *= np.float32(a)
+  w["out.2.bias"] *= np.float32(a)
+  if out.shape[1] == 2:
+    w["out.2.bias"][1] -= np.float32(a * q)
+
+
+def regime(name, weights, fwd, node_head, seed=0):
+  """A new state dict: `name` in REGIMES applied to `weights` (not modified)."""
+  w = {k: v.copy() for k, v in weights.items()}
+  if name == "R0":                       # control
+    pass
+  elif name == "R1":                     # confident head: max |l1 - l0| = 24
+    _confident_head(w, fwd, 24.0)
+  elif name == "R1x":                    # logits of ~100: exp() without max-subtraction overflows in fp32
+    a = np.float32(100.0 / np.abs(fwd(w)[0]).max())
+    w["out.2.weight"] *= a
+    w["out.2.bias"] *= a
+  elif name == "R2":                     # the reference's own init (gnn_encoder.py:343-345)
+    for l in range(N_LAYERS):
+      w[f"per_layer_out.{l}.2.weight"][:] = 0
+      w[f"per_layer_out.{l}.2.bias"][:] = 0
+  elif name == "R3":                     # U, V, A, B, C and per_layer_out.*.2 weights x 3
+    _scale_linears(w, 3.0)
+  elif name.startswith("R4_"):           # head GroupNorm input with |mean| / std = ratio
+    _offset_head_input(w, fwd, node_head, float(name[3:]))
+  elif name == "R5":                     # norm affines: gains log-uniform [0.05, 5] (4 channels at 1e-3), biases N(0,1)
+    rng = np.random.default_rng(seed)
+    for p in NORM_PREFIXES:
+      g = np.exp(rng.uniform(np.log(0.05), np.log(5.0), 256))
+      g[rng.choice(256, 4, replace=False)] = 1e-3
+      w[p + "weight"] = g.astype(np.float32)
+      w[p + "bias"] = rng.standard_normal(256).astype(np.float32)
+  elif name == "R6":                     # R3, then R4 at 10, then R1
+    _scale_linears(w, 3.0)
+    _offset_head_input(w, fwd, node_head, 10.0)
+    _confident_head(w, fwd, 24.0)
+  else:
+    raise ValueError(name)
+  return w

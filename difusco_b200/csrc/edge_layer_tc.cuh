@@ -470,28 +470,35 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
     }
     wg_bar();   // messages of all 64 rows are in shared memory
     mark(PH_E1);
-    // row-segment reduction: thread = column, rows of each 32-edge group in order (the fp32 kernel's order)
+    // row-segment reduction: thread = column, rows of each 32-edge group in order (the fp32 kernel's order).  A warp
+    // ballot over the row table marks the rows that end a (group, node) segment: the next row has another node, or is
+    // the group's last row, or lies past the last edge.  Rows past the last edge end no segment, so what they add to
+    // `run` is never stored.  The row walk then has no per-row row-table loads and no early exit, and its one branch
+    // (store the sum at a marked row) is warp-uniform.  The loops stay rolled: the kernel's code does not fit the
+    // instruction cache, and unrolling them slowed every phase.
+    const bool amax = P.agg_mode == AGG_MAX;
+    const float run0 = amax ? -INFINITY : 0.0f;
 #pragma unroll 1
     for (int g2 = 0; g2 < WG_ROWS / GROUP; ++g2) {
       const int grp = (s_base >> 5) + g2;
       if (grp >= P.g.n_groups) break;
       const int first_node = P.g.grp_first[grp];
       const size_t pair_base = (size_t)P.g.grp_pair[grp];
-#pragma unroll
+      const int node = w_row[g2 * GROUP + lane];   // -1 past the last edge
+      const int nxt = __shfl_down_sync(0xffffffffu, node, 1);
+      const uint32_t ends = __ballot_sync(0xffffffffu, node >= 0 && (lane == GROUP - 1 || nxt != node));
+#pragma unroll 1
       for (int cc = 0; cc < 2; ++cc) {
         const int c = tid + 128 * cc;
-        float run = (P.agg_mode == AGG_MAX) ? -INFINITY : 0.0f;
-#pragma unroll 4
+        float run = run0;
+#pragma unroll 8
         for (int r = 0; r < GROUP; ++r) {
           const int lr = g2 * GROUP + r;
-          const int node = w_row[lr];
-          if (node < 0) break;
           const float m = msg[lr * H + (c ^ (8 * (lr & 7)))];
-          run = (P.agg_mode == AGG_MAX) ? fmaxf(run, m) : run + m;
-          const int nxt = (r + 1 < GROUP) ? w_row[lr + 1] : -1;
-          if (nxt != node) {
-            P.partials[(pair_base + (size_t)(node - first_node)) * H + c] = run;
-            run = (P.agg_mode == AGG_MAX) ? -INFINITY : 0.0f;
+          run = amax ? fmaxf(run, m) : run + m;
+          if ((ends >> r) & 1u) {
+            P.partials[(pair_base + (size_t)(w_row[lr] - first_node)) * H + c] = run;
+            run = run0;
           }
         }
       }

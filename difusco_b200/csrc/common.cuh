@@ -68,9 +68,6 @@ struct LayerParams {
   const float* ln_o_g; const float* ln_o_b;   // per_layer_out.0
   const float* Wt_tau;    // [128][256]   in-major, time_embed_layers.l.1
   const float* b_tau;     // [256]
-  // bf16 hi/lo splits of C and O for the tensor-core kernel: [out 256][in 256] K-major
-  const uint16_t* C_hi; const uint16_t* C_lo;
-  const uint16_t* O_hi; const uint16_t* O_lo;
 };
 
 // The prepared graph (device pointers), sorted by row.

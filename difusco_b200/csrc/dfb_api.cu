@@ -22,9 +22,14 @@ using namespace dfb;
 
 static std::string g_create_error;
 
+// A device allocation owned by the context (grown by ensure()), freed with it.
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { if (p) cudaFree(p); }
 };
 
 struct dfb_ctx {
@@ -35,6 +40,7 @@ struct dfb_ctx {
   int L = 0, out_channels = 0, node_only = 0;
   int agg_mode = AGG_SUM;
   int edge_impl = DFB_EDGE_IMPL_TC;
+  bool phase_timing = false;   // edge layers of the product kernel run through its timed copy (dfb_set_phase_timing)
   DevBuf wbuf, wbuf16, layers_dev;
   std::vector<LayerParams> layers;
   TimeParams tp{};
@@ -86,6 +92,21 @@ struct dfb_ctx {
   std::vector<cudaEvent_t> ev_pool;
   size_t ev_used = 0;
   TcState tc;
+
+  // Releases whatever has been created so far: dfb_destroy, and every failure exit of dfb_create.  The device
+  // buffers and the tensor-core state release themselves.
+  ~dfb_ctx() {
+    for (cudaEvent_t ev : ev_pool) cudaEventDestroy(ev);
+    if (loop_exec) cudaGraphExecDestroy(loop_exec);
+    if (loop_stream) cudaStreamDestroy(loop_stream);
+    if (loop_in) cudaEventDestroy(loop_in);
+    if (loop_out) cudaEventDestroy(loop_out);
+    for (int i = 0; i < STAGE_SLOTS; ++i) {
+      if (h_tvals[i]) cudaFreeHost(h_tvals[i]);
+      if (h_steps[i]) cudaFreeHost(h_steps[i]);
+      if (stage_ev[i]) cudaEventDestroy(stage_ev[i]);
+    }
+  }
 };
 
 #define FAIL(ctx, code, ...)                         \
@@ -221,25 +242,6 @@ extern "C" int dfb_create(dfb_ctx** out, int device) {
 extern "C" int dfb_destroy(dfb_ctx* ctx) {
   if (!ctx) return DFB_OK;
   cudaSetDevice(ctx->device);
-  DevBuf* bufs[] = {&ctx->wbuf, &ctx->wbuf16, &ctx->layers_dev, &ctx->d_row, &ctx->d_col, &ctx->d_perm,
-                    &ctx->d_rowptr, &ctx->d_grp_first, &ctx->d_grp_pair, &ctx->d_ei_stage, &ctx->e, &ctx->h,
-                    &ctx->h0, &ctx->uvab, &ctx->uvab0, &ctx->partials, &ctx->feat, &ctx->tvec, &ctx->tvals,
-                    &ctx->gn_part, &ctx->gn_stats, &ctx->d_points, &ctx->d_xt, &ctx->d_u, &ctx->opt_points, &ctx->opt_tours,
-                    &ctx->opt_pos, &ctx->opt_dnext, &ctx->opt_cand, &ctx->opt_tiles, &ctx->opt_state, &ctx->opt_best};
-  for (DevBuf* b : bufs)
-    if (b->p) cudaFree(b->p);
-  for (cudaEvent_t ev : ctx->ev_pool) cudaEventDestroy(ev);
-  if (ctx->loop_exec) cudaGraphExecDestroy(ctx->loop_exec);
-  if (ctx->loop_stream) cudaStreamDestroy(ctx->loop_stream);
-  if (ctx->loop_in) cudaEventDestroy(ctx->loop_in);
-  if (ctx->loop_out) cudaEventDestroy(ctx->loop_out);
-  if (ctx->d_steps.p) cudaFree(ctx->d_steps.p);
-  for (int i = 0; i < dfb_ctx::STAGE_SLOTS; ++i) {
-    if (ctx->h_tvals[i]) cudaFreeHost(ctx->h_tvals[i]);
-    if (ctx->h_steps[i]) cudaFreeHost(ctx->h_steps[i]);
-    if (ctx->stage_ev[i]) cudaEventDestroy(ctx->stage_ev[i]);
-  }
-  tc_destroy(&ctx->tc);
   delete ctx;
   return DFB_OK;
 }
@@ -322,7 +324,14 @@ extern "C" int dfb_load_weights(dfb_ctx* ctx, int n_layers, int hidden_dim, int 
     size_t Wt_uvab, b_uvab, Wt_C, Wt_O, b_O, hg, hb, eg, eb, og, ob, Wt_tau, b_tau;
   };
   std::vector<LOff> lo(L);
-  std::vector<uint16_t> arena16((size_t)(L * 12 + 4) * H * H);
+  std::vector<uint16_t> arena16((size_t)w_arena_rows(L) * H);
+  auto put16 = [&](const float* W, int row) {   // W [256 out][256 in] -> bf16 hi, lo at arena row `row`, K-major
+    uint16_t* hi = &arena16[(size_t)row * H];
+    for (int i = 0; i < H * H; ++i) {
+      hi[i] = f2bf16_rn(W[i]);
+      hi[W_LO_ROWS * H + i] = f2bf16_rn(W[i] - bf16_to_f(hi[i]));
+    }
+  };
   const float* p;
   for (int l = 0; l < L; ++l) {
     std::string pre = "layers." + std::to_string(l) + ".";
@@ -356,36 +365,14 @@ extern "C" int dfb_load_weights(dfb_ctx* ctx, int n_layers, int hidden_dim, int 
     std::string pt = "time_embed_layers." + std::to_string(l) + ".1.";
     GET(pt + "weight", H * TE, &p); lo[l].Wt_tau = put_T(p, H, TE);
     GET(pt + "bias", H, &p);        lo[l].b_tau = put_v(p, H);
-    // bf16 hi/lo split of C and O, [out][in] K-major (the tensor-core B operand)
-    uint16_t* a16 = &arena16[(size_t)l * 12 * H * H];
-    for (int i = 0; i < H * H; ++i) {
-      uint16_t hi = f2bf16_rn(WC[i]);
-      a16[i] = hi;
-      a16[H * H + i] = f2bf16_rn(WC[i] - bf16_to_f(hi));
-      hi = f2bf16_rn(WO[i]);
-      a16[2 * H * H + i] = hi;
-      a16[3 * H * H + i] = f2bf16_rn(WO[i] - bf16_to_f(hi));
-      for (int qq = 0; qq < 4; ++qq) {   // U, V, A, B: [out][in] K-major, hi then lo
-        hi = f2bf16_rn(W[qq][i]);
-        a16[(size_t)(4 + 2 * qq) * H * H + i] = hi;
-        a16[(size_t)(5 + 2 * qq) * H * H + i] = f2bf16_rn(W[qq][i] - bf16_to_f(hi));
-      }
-    }
+    put16(WC, w_row_C(l));
+    put16(WO, w_row_O(l));
+    for (int q = 0; q < 4; ++q) put16(W[q], w_row_UVAB(l) + q * W_MAT_ROWS);
   }
   size_t o_node_W, o_node_b, o_edge_W, o_edge_b, o_t0W, o_t0b, o_t2W, o_t2b, o_gng, o_gnb, o_outW, o_outb;
-  GET("node_embed.weight", H * H, &p); o_node_W = put_T(p, H, H);
-  for (int i = 0; i < H * H; ++i) {
-    uint16_t hi = f2bf16_rn(p[i]);
-    arena16[(size_t)(L * 12 + 2) * H * H + i] = hi;
-    arena16[(size_t)(L * 12 + 3) * H * H + i] = f2bf16_rn(p[i] - bf16_to_f(hi));
-  }
+  GET("node_embed.weight", H * H, &p); o_node_W = put_T(p, H, H); put16(p, w_row_embed(L, 1));
   GET("node_embed.bias", H, &p);       o_node_b = put_v(p, H);
-  GET("edge_embed.weight", H * H, &p); o_edge_W = put_T(p, H, H);
-  for (int i = 0; i < H * H; ++i) {
-    uint16_t hi = f2bf16_rn(p[i]);
-    arena16[(size_t)(L * 12 + 0) * H * H + i] = hi;
-    arena16[(size_t)(L * 12 + 1) * H * H + i] = f2bf16_rn(p[i] - bf16_to_f(hi));
-  }
+  GET("edge_embed.weight", H * H, &p); o_edge_W = put_T(p, H, H); put16(p, w_row_embed(L, 0));
   GET("edge_embed.bias", H, &p);       o_edge_b = put_v(p, H);
   GET("time_embed.0.weight", TE * H, &p); o_t0W = put_T(p, TE, H);
   GET("time_embed.0.bias", TE, &p);       o_t0b = put_v(p, TE);
@@ -421,7 +408,6 @@ extern "C" int dfb_load_weights(dfb_ctx* ctx, int n_layers, int hidden_dim, int 
   CK(ctx, cudaMemcpy(ctx->wbuf.p, arena.data(), arena.size() * sizeof(float), cudaMemcpyHostToDevice));
   CK(ctx, cudaMemcpy(ctx->wbuf16.p, arena16.data(), arena16.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
   const float* base = (const float*)ctx->wbuf.p;
-  const uint16_t* base16 = (const uint16_t*)ctx->wbuf16.p;
   ctx->layers.resize(L);
   for (int l = 0; l < L; ++l) {
     LayerParams& lp = ctx->layers[l];
@@ -431,8 +417,6 @@ extern "C" int dfb_load_weights(dfb_ctx* ctx, int n_layers, int hidden_dim, int 
     lp.ln_e_g = base + lo[l].eg; lp.ln_e_b = base + lo[l].eb;
     lp.ln_o_g = base + lo[l].og; lp.ln_o_b = base + lo[l].ob;
     lp.Wt_tau = base + lo[l].Wt_tau; lp.b_tau = base + lo[l].b_tau;
-    lp.C_hi = base16 + (size_t)l * 12 * H * H; lp.C_lo = lp.C_hi + H * H;
-    lp.O_hi = lp.C_hi + 2 * H * H;            lp.O_lo = lp.C_hi + 3 * H * H;
   }
   CK(ctx, cudaMemcpy(ctx->layers_dev.p, ctx->layers.data(), L * sizeof(LayerParams), cudaMemcpyHostToDevice));
   ctx->Wt_node = base + o_node_W; ctx->b_node = base + o_node_b;
@@ -446,7 +430,7 @@ extern "C" int dfb_load_weights(dfb_ctx* ctx, int n_layers, int hidden_dim, int 
   ctx->cl0 = (float*)ctx->wbuf.p + o_cl0;   // second half stays zero (arena slots are zero-initialised)
   ctx->L = L; ctx->out_channels = out_channels; ctx->node_only = node_feature_only;
 
-  int r = tc_bind_weights(&ctx->tc, ctx->layers.data(), L);
+  int r = tc_bind_weights(&ctx->tc, (const uint16_t*)ctx->wbuf16.p, L);
   if (r) FAIL(ctx, DFB_E_CUDA, "tensor-map setup failed: %s", ctx->tc.err.c_str());
 
   // categorical edge-embedding LUT: edge_embed(edge_pos_embed(x)) for x in {0, 1}
@@ -588,39 +572,40 @@ extern "C" int dfb_prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_
   return DFB_OK;
 }
 
-// node-side linears h -> [U|V|A|B] h of layer l: tensor-core path (product) or fp32 FFMA (validation impl)
-static int node_linears(dfb_ctx* ctx, int l, const float* h, float* uvab, int V, cudaStream_t st) {
-  if (ctx->edge_impl == DFB_EDGE_IMPL_FP32) {
-    dim3 grid((V + LIN_ROWS - 1) / LIN_ROWS, 4);
-    k_linear<<<grid, 256, 0, st>>>(h, ctx->layers[l].Wt_uvab, ctx->layers[l].b_uvab, uvab, V, 4 * H);
+// What dfb_set_edge_impl selects for the linears and edge layers: the fp32 FFMA kernels (validation), or the
+// tensor-core kernels with nwg consumer warpgroups per edge-layer CTA (tc 2, tc1 1; under fp32 the GEMM1 dump of
+// dfb_debug_edge_gemm uses 2).
+struct EdgeImpl { bool fp32; int nwg; };
+static EdgeImpl edge_impl(const dfb_ctx* ctx) {
+  return {ctx->edge_impl == DFB_EDGE_IMPL_FP32, ctx->edge_impl == DFB_EDGE_IMPL_TC1 ? 1 : 2};
+}
+
+// rows X[R][256] -> Y = X W^T + b: fp32 FFMA (Wt in-major [256][N]) or the tensor-core linear (N / 256 matrices of the
+// bf16 arena from row w_row on).  One launch either way.
+static int linear_rows(dfb_ctx* ctx, const float* X, const float* Wt, int w_row, const float* b, float* Y, int R, int N,
+                       cudaStream_t st) {
+  if (edge_impl(ctx).fp32) {
+    dim3 grid((R + LIN_ROWS - 1) / LIN_ROWS, N / 256);
+    k_linear<<<grid, 256, 0, st>>>(X, Wt, b, Y, R, N);
     CKL(ctx);
     return DFB_OK;
   }
-  int r = tc_launch_linear(&ctx->tc, l * 12 * H + 4 * H, 4, h, uvab, ctx->layers[l].b_uvab, V, ctx->g, ctx->layers[l], st);
-  if (r) FAIL(ctx, DFB_E_CUDA, "tensor-core node linear: %s", ctx->tc.err.c_str());
-  ctx->launches += 1;
+  if (tc_launch_linear(&ctx->tc, X, Y, b, R, N / H, w_row, st))
+    FAIL(ctx, DFB_E_CUDA, "tensor-core linear: %s", ctx->tc.err.c_str());
+  ctx->launches++;
   return DFB_OK;
 }
 
-// rows X[R][256] -> Y = X Wt + b through the generic linear, chunked features
-static int linear_rows(dfb_ctx* ctx, const float* X, const float* Wt, const float* b, float* Y, int R, int N,
-                       cudaStream_t st) {
-  dim3 grid((R + LIN_ROWS - 1) / LIN_ROWS, N / 256);
-  k_linear<<<grid, 256, 0, st>>>(X, Wt, b, Y, R, N);
-  CKL(ctx);
-  return DFB_OK;
+// node-side linears h -> [U|V|A|B] h of layer l
+static int node_linears(dfb_ctx* ctx, int l, const float* h, float* uvab, int V, cudaStream_t st) {
+  const LayerParams& lp = ctx->layers[l];
+  return linear_rows(ctx, h, lp.Wt_uvab, w_row_UVAB(l), lp.b_uvab, uvab, V, 4 * H, st);
 }
 
-// embedding linears (256 -> 256): which = 0 edge_embed, 1 node_embed.  Tensor-core path unless the fp32 validation
-// implementation is selected.
+// embedding linears (256 -> 256): which = 0 edge_embed, 1 node_embed
 static int embed_rows(dfb_ctx* ctx, int which, const float* X, float* Y, int R, cudaStream_t st) {
-  if (ctx->edge_impl == DFB_EDGE_IMPL_FP32 || !ctx->graph_ready)
-    return linear_rows(ctx, X, which ? ctx->Wt_node : ctx->Wt_edge, which ? ctx->b_node : ctx->b_edge, Y, R, H, st);
-  int r = tc_launch_linear(&ctx->tc, (ctx->L * 12 + 2 * which) * H, 1, X, Y, which ? ctx->b_node : ctx->b_edge, R, ctx->g,
-                           ctx->layers[0], st);
-  if (r) FAIL(ctx, DFB_E_CUDA, "tensor-core embedding linear: %s", ctx->tc.err.c_str());
-  ctx->launches += 1;
-  return DFB_OK;
+  return linear_rows(ctx, X, which ? ctx->Wt_node : ctx->Wt_edge, w_row_embed(ctx->L, which),
+                     which ? ctx->b_node : ctx->b_edge, Y, R, H, st);
 }
 
 extern "C" int dfb_set_points(dfb_ctx* ctx, const float* points, void* stream_) {
@@ -669,7 +654,8 @@ static int launch_edge_layer(dfb_ctx* ctx, int l, const float* uvab, const float
     ev1 = ctx->ev_pool[ctx->ev_used++];
     CK(ctx, cudaEventRecord(ev0, st));
   }
-  if (ctx->edge_impl == DFB_EDGE_IMPL_FP32) {
+  const EdgeImpl impl = edge_impl(ctx);
+  if (impl.fp32) {
     if (e_zero) CK(ctx, cudaMemsetAsync(ctx->e.p, 0, (size_t)ctx->g.E * H * sizeof(float), st));
     if (xt_for_lut) {
       k_lut_expand<<<(ctx->g.E + 3) / 4, 256, 0, st>>>(xt_for_lut, ctx->g.perm, ctx->lut, (float*)ctx->e.p, ctx->g.E);
@@ -680,11 +666,11 @@ static int launch_edge_layer(dfb_ctx* ctx, int l, const float* uvab, const float
                                                             ctx->agg_mode);
     CKL(ctx);
   } else {
-    int r = tc_launch_edge_layer(&ctx->tc, l, (float*)ctx->e.p, uvab, (float*)ctx->partials.p, ctx->g,
-                                 ctx->layers[l], tvec_edge, write_e, e_zero, xt_for_lut, ctx->lut,
-                                 ctx->agg_mode, st, ctx->edge_impl == DFB_EDGE_IMPL_TC1 ? 1 : 2);
-    if (r) FAIL(ctx, DFB_E_CUDA, "tensor-core edge layer: %s", ctx->tc.err.c_str());
-    ctx->launches += ctx->tc.last_launches;
+    if (tc_launch_edge_layer(&ctx->tc, l, (float*)ctx->e.p, uvab, (float*)ctx->partials.p, ctx->g, ctx->layers[l],
+                             tvec_edge, write_e, e_zero, xt_for_lut, ctx->lut, ctx->agg_mode, impl.nwg,
+                             ctx->phase_timing, nullptr, st))
+      FAIL(ctx, DFB_E_CUDA, "tensor-core edge layer: %s", ctx->tc.err.c_str());
+    ctx->launches++;
   }
   if (ctx->profiling) CK(ctx, cudaEventRecord(ev1, st));
   return DFB_OK;
@@ -895,7 +881,7 @@ extern "C" int dfb_denoise(dfb_ctx* ctx, int diffusion_type, float* xt, int step
   if (want_graph) {
     dfb_ctx::LoopKey key;
     key.buf_gen = ctx->buf_gen; key.steps = steps; key.diffusion = diffusion_type; key.impl = ctx->edge_impl;
-    key.agg = ctx->agg_mode; key.timed = ctx->tc.timed; key.uniforms = uniforms;
+    key.agg = ctx->agg_mode; key.timed = ctx->phase_timing; key.uniforms = uniforms;
     if (!ctx->loop_exec || !(ctx->loop_key == key)) {
       if (ctx->loop_exec) {
         cudaGraphExecDestroy(ctx->loop_exec);
@@ -947,7 +933,7 @@ extern "C" int dfb_set_graph_capture(dfb_ctx* ctx, int enabled) {
 
 extern "C" int dfb_set_phase_timing(dfb_ctx* ctx, int enabled) {
   if (!ctx) return DFB_E_INVALID;
-  ctx->tc.timed = enabled != 0;   // part of the captured loop's key: the next dfb_denoise re-captures
+  ctx->phase_timing = enabled != 0;   // part of the captured loop's key: the next dfb_denoise re-captures
   return DFB_OK;
 }
 
@@ -1008,13 +994,11 @@ extern "C" int dfb_debug_edge_gemm(dfb_ctx* ctx, int layer, const float* e_in, f
   CK(ctx, cudaSetDevice(ctx->device));
   if (!ctx->graph_ready) FAIL(ctx, DFB_E_INVALID, "dfb_prepare_graph must be called first");
   if (layer < 0 || layer >= ctx->L) FAIL(ctx, DFB_E_INVALID, "layer out of range");
-  ctx->tc.debug_acc = acc_out;
-  int r = tc_launch_edge_layer(&ctx->tc, layer, const_cast<float*>(e_in), (const float*)ctx->uvab.p,
-                               (float*)ctx->partials.p, ctx->g, ctx->layers[layer], nullptr, 0, 0, nullptr,
-                               ctx->lut, AGG_SUM, st, ctx->edge_impl == DFB_EDGE_IMPL_TC1 ? 1 : 2);
-  ctx->tc.debug_acc = nullptr;
-  if (r) FAIL(ctx, DFB_E_CUDA, "tensor-core edge layer: %s", ctx->tc.err.c_str());
-  ctx->launches += 1;
+  if (tc_launch_edge_layer(&ctx->tc, layer, const_cast<float*>(e_in), (const float*)ctx->uvab.p,
+                           (float*)ctx->partials.p, ctx->g, ctx->layers[layer], nullptr, 0, 0, nullptr, ctx->lut, AGG_SUM,
+                           edge_impl(ctx).nwg, false, acc_out, st))
+    FAIL(ctx, DFB_E_CUDA, "tensor-core edge layer: %s", ctx->tc.err.c_str());
+  ctx->launches++;
   return DFB_OK;
 }
 

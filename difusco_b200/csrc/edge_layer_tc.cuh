@@ -44,6 +44,19 @@ constexpr int TC_A_BYTES = 8 * TC_A_CHUNK;      // 4 K-chunks x (hi, lo) per war
 constexpr int CONV_BATCH = 16;   // conversion: float4 row loads of 32
 constexpr int E4_BATCH = 16;     // E4: float2 e_in loads of a row half of 32
 
+// The bf16 weight arena, the tensor-core kernels' B operand: every row offset into it comes from here.
+// Each 256x256 matrix W [out][in] takes two blocks of 256 rows, K-major: hi = bf16(W), then lo = bf16(W - hi).
+// Layer l holds C, O, U, V, A, B in that order; edge_embed and node_embed follow the L layers.  One 2-D tensor map
+// covers the whole arena, so a matrix is addressed by the arena row of its hi block.
+constexpr int W_LO_ROWS = H;                   // a matrix's hi block -> its lo block
+constexpr int W_MAT_ROWS = 2 * W_LO_ROWS;      // one matrix -> the next
+constexpr int W_LAYER_ROWS = 6 * W_MAT_ROWS;   // C, O, U, V, A, B
+__host__ __device__ constexpr int w_row_C(int l) { return l * W_LAYER_ROWS; }
+__host__ __device__ constexpr int w_row_O(int l) { return w_row_C(l) + W_MAT_ROWS; }
+__host__ __device__ constexpr int w_row_UVAB(int l) { return w_row_C(l) + 2 * W_MAT_ROWS; }   // U, V, A, B, W_MAT_ROWS apart
+__host__ __device__ constexpr int w_row_embed(int L, int which) { return L * W_LAYER_ROWS + which * W_MAT_ROWS; }   // 0 edge, 1 node
+__host__ __device__ constexpr int w_arena_rows(int L) { return w_row_embed(L, 2); }
+
 template <int NWG>
 struct TcCfg {
   static_assert(NWG == 1 || NWG == 2, "one or two consumer warpgroups");
@@ -78,11 +91,11 @@ struct TcParams {
   const float* lin_bias;
   int lin_rows;
   int lin_nb;             // 256-column output blocks per row tile: 4 (U|V|A|B) or 1 (embedding linears)
-  int lin_w_row;          // first weight row of block 0 in the bf16 arena (blocks are 512 rows apart: hi, lo)
+  int lin_w_row;          // arena row of block 0 (blocks are W_MAT_ROWS apart)
   int* error_flag;
   unsigned long long* phase_cycles;   // [32] phase timers (k_edge_layer_wg2_timed only), see PH_*
   int write_e, e_zero, agg_mode;
-  int w_row_base;         // row of this layer's C_hi block in the bf16 weight arena tensor map
+  int w_row_base;         // arena row of this layer's C (w_row_C)
   int n_tiles;
 };
 
@@ -283,9 +296,10 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
           const int s = u % NSTAGE;
           mbar_wait(&empty[s], ((u / NSTAGE) & 1) ^ 1, P.error_flag, 1);
           mbar_arrive_expect_tx(&full[s], TC_B_BYTES);
-          // C_hi,C_lo | O_hi,O_lo blocks of 256 rows; linear mode: U|V|A|B (hi,lo) blocks 512 rows apart
-          const int row = (lin ? P.lin_w_row + (P.lin_nb == 4 ? (tile & 3) : 0) * 512 : P.w_row_base + (i >= 8 ? 512 : 0)) +
-                          (i & 1) * 256;
+          // hi, lo of C, then of O; linear mode: hi, lo of block (tile & 3) of U|V|A|B, or of the one embedding
+          const int row = (lin ? P.lin_w_row + (P.lin_nb == 4 ? (tile & 3) : 0) * W_MAT_ROWS
+                               : P.w_row_base + (i >= 8 ? w_row_O(0) - w_row_C(0) : 0)) +
+                          (i & 1) * W_LO_ROWS;
           tma_load_2d(smem_base + Cfg::OFF_B + s * TC_B_BYTES, &wmap, &full[s], ((i >> 1) & 3) * TC_KCH, row);
         }
       }
@@ -614,22 +628,25 @@ k_linear_wg2(const __grid_constant__ CUtensorMap wmap, const TcParams P) {
 // ----------------------------------------------------------------------------------------------
 // host side
 // ----------------------------------------------------------------------------------------------
+// What the tensor-core kernels keep for the life of a context; everything else is an argument of one launch.
 struct TcState {
   std::string err;
   int num_sms = 0;
   CUtensorMap wmap;
   bool bound = false;
-  int last_launches = 0;
   float* zero_row = nullptr;
   int* error_flag = nullptr;    // device alias of error_host (host-mapped: readable after a trap)
   int* error_host = nullptr;
-  float* debug_acc = nullptr;   // set by the debug entry point for one launch
-  const float* lin_in = nullptr;   // linear mode arguments, set for one launch by tc_launch_linear
-  float* lin_out = nullptr;
-  const float* lin_bias = nullptr;
-  int lin_rows = 0, lin_nb = 4, lin_w_row = 0;
   unsigned long long* phase_cycles = nullptr;   // [32] dfb_debug_phase_cycles; only the timed kernel adds to it
-  bool timed = false;                           // product launches go to k_edge_layer_wg2_timed
+
+  TcState() = default;
+  TcState(const TcState&) = delete;
+  TcState& operator=(const TcState&) = delete;
+  ~TcState() {
+    if (zero_row) cudaFree(zero_row);
+    if (error_host) cudaFreeHost(error_host);
+    if (phase_cycles) cudaFree(phase_cycles);
+  }
 };
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -661,19 +678,9 @@ inline int tc_init(TcState* st, int num_sms) {
   return 0;
 }
 
-inline void tc_destroy(TcState* st) {
-  if (st->zero_row) cudaFree(st->zero_row);
-  if (st->error_host) cudaFreeHost(st->error_host);
-  if (st->phase_cycles) cudaFree(st->phase_cycles);
-  st->zero_row = nullptr;
-  st->error_flag = nullptr;
-  st->error_host = nullptr;
-}
-
-// One tensor map over the whole bf16 weight arena: [L*12*256 rows][256 K], rows of layer l are
-// C_hi | C_lo | O_hi | O_lo | U_hi | U_lo | V_hi | V_lo | A_hi | A_lo | B_hi | B_lo (256 rows each); after the
-// layers: edge_embed hi | lo, node_embed hi | lo.  Box = 64 K x 256 rows, 128-byte swizzle.
-inline int tc_bind_weights(TcState* st, const LayerParams* layers, int L) {
+// One tensor map over the whole bf16 weight arena at `arena` (w_arena_rows(L) rows of 256 K, layout above).
+// Box = 64 K x 256 rows, 128-byte swizzle.
+inline int tc_bind_weights(TcState* st, const uint16_t* arena, int L) {
   void* fn = nullptr;
   cudaDriverEntryPointQueryResult qres;
   cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres);
@@ -682,11 +689,11 @@ inline int tc_bind_weights(TcState* st, const LayerParams* layers, int L) {
     cudaGetLastError();
     return -2;
   }
-  cuuint64_t gdim[2] = {(cuuint64_t)H, (cuuint64_t)(L * 12 + 4) * H};
+  cuuint64_t gdim[2] = {(cuuint64_t)H, (cuuint64_t)w_arena_rows(L)};
   cuuint64_t gstride[1] = {(cuuint64_t)H * sizeof(uint16_t)};
   cuuint32_t box[2] = {(cuuint32_t)TC_KCH, 256u};
   cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = ((PFN_encodeTiled)fn)(&st->wmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)layers[0].C_hi, gdim,
+  CUresult r = ((PFN_encodeTiled)fn)(&st->wmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)arena, gdim,
                                      gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -697,52 +704,51 @@ inline int tc_bind_weights(TcState* st, const LayerParams* layers, int L) {
   return 0;
 }
 
-// nwg: consumer warpgroups per CTA (2: product kernel, 1: the 64-row-tile variant)
-inline int tc_launch_edge_layer(TcState* st, int l, float* e, const float* uvab, float* partials, GraphDev g,
-                                LayerParams lp, const float* tvec_edge, int write_e, int e_zero,
-                                const float* xt_lut, const float* lut, int agg_mode, cudaStream_t stream, int nwg = 2) {
-  st->last_launches = 0;
+// Launches `kernel` over tiles of TcCfg<NWG>::TILE rows of `rows` rows (times nb column blocks), persistent: one CTA
+// per SM, fewer when there are fewer tiles.  P holds the launch's own arguments; the context's are added here.
+template <int NWG>
+inline int tc_launch(TcState* st, void (*kernel)(CUtensorMap, TcParams), TcParams& P, int rows, int nb,
+                     cudaStream_t stream) {
   if (!st->bound) {
     st->err = "weights not bound";
     return -1;
   }
-  if (st->lin_out) nwg = 2;
-  const int tile_rows = nwg * WG_ROWS;
-  TcParams P;
-  P.e = e; P.uvab = uvab; P.partials = partials; P.g = g; P.lp = lp; P.tvec = tvec_edge;
-  P.xt_lut = xt_lut; P.lut = lut; P.zero_row = st->zero_row; P.debug_acc = st->debug_acc;
-  P.error_flag = st->error_flag;
-  P.phase_cycles = st->phase_cycles;
-  P.write_e = (st->debug_acc || st->lin_out) ? 0 : write_e;
-  P.e_zero = e_zero; P.agg_mode = agg_mode;
-  P.w_row_base = l * 12 * H;
-  P.lin_in = st->lin_in; P.lin_out = st->lin_out; P.lin_bias = st->lin_bias; P.lin_rows = st->lin_rows;
-  P.lin_nb = st->lin_nb; P.lin_w_row = st->lin_w_row;
-  P.n_tiles = st->lin_out ? st->lin_nb * ((st->lin_rows + tile_rows - 1) / tile_rows) : (g.E + tile_rows - 1) / tile_rows;
+  P.zero_row = st->zero_row; P.error_flag = st->error_flag; P.phase_cycles = st->phase_cycles;
+  P.n_tiles = nb * ((rows + TcCfg<NWG>::TILE - 1) / TcCfg<NWG>::TILE);
   const int grid = P.n_tiles < st->num_sms ? P.n_tiles : st->num_sms;
-  if (st->lin_out) k_linear_wg2<<<grid, TcCfg<2>::THREADS, TcCfg<2>::SMEM_ALLOC, stream>>>(st->wmap, P);
-  else if (nwg == 1) k_edge_layer_wg1<<<grid, TcCfg<1>::THREADS, TcCfg<1>::SMEM_ALLOC, stream>>>(st->wmap, P);
-  else if (st->timed && !st->debug_acc)
-    k_edge_layer_wg2_timed<<<grid, TcCfg<2>::THREADS, TcCfg<2>::SMEM_ALLOC, stream>>>(st->wmap, P);
-  else k_edge_layer_wg2<<<grid, TcCfg<2>::THREADS, TcCfg<2>::SMEM_ALLOC, stream>>>(st->wmap, P);
-  cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) {
-    st->err = std::string("launch: ") + cudaGetErrorString(err);
-    return -2;
-  }
-  st->last_launches = 1;
-  return 0;
+  kernel<<<grid, TcCfg<NWG>::THREADS, TcCfg<NWG>::SMEM_ALLOC, stream>>>(st->wmap, P);
+  const cudaError_t err = cudaGetLastError();
+  if (err == cudaSuccess) return 0;
+  st->err = std::string("launch: ") + cudaGetErrorString(err);
+  return -2;
 }
 
-// Generic [rows][256] x (nb blocks of 256x256, bf16 hi/lo at arena rows w_row + 512 b) -> [rows][nb*256] (+ bias) on the
-// tensor-core path.  nb = 4: the node-side linears U|V|A|B of a layer; nb = 1: node / edge embedding linears.
-inline int tc_launch_linear(TcState* st, int w_row, int nb, const float* in, float* out, const float* bias, int rows,
-                            GraphDev g, LayerParams lp, cudaStream_t stream) {
-  st->lin_in = in; st->lin_out = out; st->lin_bias = bias; st->lin_rows = rows; st->lin_nb = nb; st->lin_w_row = w_row;
-  int r = tc_launch_edge_layer(st, 0, const_cast<float*>(in), nullptr, nullptr, g, lp, nullptr, 0, 0, nullptr, nullptr,
-                               AGG_SUM, stream);
-  st->lin_in = nullptr; st->lin_out = nullptr; st->lin_bias = nullptr; st->lin_rows = 0;
-  return r;
+// One fused edge layer l over graph g.  nwg 2: k_edge_layer_wg2, the product kernel, or with `timed` its copy with
+// phase timers, k_edge_layer_wg2_timed; nwg 1: k_edge_layer_wg1, the 64-row-tile variant.  A non-null debug_acc
+// (tests) runs GEMM1 only and writes its accumulator [E][256] there, never through the timed copy.
+inline int tc_launch_edge_layer(TcState* st, int l, float* e, const float* uvab, float* partials, const GraphDev& g,
+                                const LayerParams& lp, const float* tvec, int write_e, int e_zero, const float* xt_lut,
+                                const float* lut, int agg_mode, int nwg, bool timed, float* debug_acc,
+                                cudaStream_t stream) {
+  TcParams P{};
+  P.e = e; P.uvab = uvab; P.partials = partials; P.g = g; P.lp = lp; P.tvec = tvec;
+  P.xt_lut = xt_lut; P.lut = lut; P.debug_acc = debug_acc;
+  P.write_e = debug_acc ? 0 : write_e;
+  P.e_zero = e_zero; P.agg_mode = agg_mode;
+  P.w_row_base = w_row_C(l);
+  if (nwg == 1) return tc_launch<1>(st, k_edge_layer_wg1, P, g.E, 1, stream);
+  return tc_launch<2>(st, timed && !debug_acc ? k_edge_layer_wg2_timed : k_edge_layer_wg2, P, g.E, 1, stream);
+}
+
+// in [rows][256] times nb 256x256 matrices of the arena, the first at row w_row (w_row_*), -> out [rows][nb * 256]
+// + bias, on k_linear_wg2: the node linears U|V|A|B of a layer (nb 4) or an embedding linear (nb 1).
+inline int tc_launch_linear(TcState* st, const float* in, float* out, const float* bias, int rows, int nb, int w_row,
+                            cudaStream_t stream) {
+  TcParams P{};
+  P.lin_in = in; P.lin_out = out; P.lin_bias = bias; P.lin_rows = rows; P.lin_nb = nb; P.lin_w_row = w_row;
+  // the kernel stages a layer's vectors in every mode; linear mode reads none of them
+  P.lp.ln_e_g = P.lp.ln_e_b = P.lp.ln_o_g = P.lp.ln_o_b = P.lp.b_O = st->zero_row;
+  return tc_launch<2>(st, k_linear_wg2, P, rows, nb, stream);
 }
 
 }  // namespace dfb

@@ -225,6 +225,19 @@ __device__ __forceinline__ float quad_sum(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 1);
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
+// Exchanges the accumulator fragment's two row halves (acc[4 j], acc[4 j + 1] <-> acc[4 j + 2], acc[4 j + 3]).  An
+// epilogue loop over the row half h works on acc[4 j] and acc[4 j + 1] only and calls this at the end of each pass: two
+// passes leave the fragment in its original order.
+__device__ __forceinline__ void swap_row_halves(float (&d)[128]) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const float x0 = d[4 * j], x1 = d[4 * j + 1];
+    d[4 * j] = d[4 * j + 2];
+    d[4 * j + 1] = d[4 * j + 3];
+    d[4 * j + 2] = x0;
+    d[4 * j + 3] = x1;
+  }
+}
 
 // Phase timers of the instrumented entry point k_edge_layer_wg2_timed: slots of TcParams::phase_cycles, summed over
 // every consumer warpgroup of the launch (SM clock cycles read by thread 0 of the warpgroup).  The phases partition the
@@ -249,9 +262,15 @@ enum {
 //   acc[4 j + 2 h + b]  ->  row 16 wi + g + 8 h,  column 8 j + 2 t + b        (j < 32, h, b in {0, 1})
 // so the 256 columns of a row are spread over the 4 threads of a quad: row reductions are 64 thread-local terms
 // plus two shuffles.
+//
+// Code size is part of this kernel's speed: each consumer warp runs the whole tile body once per tile, so a body larger
+// than the instruction cache is fetched again on every tile (DESIGN §4.2).  E1 and E2 / E3 therefore loop over the row
+// half h with `#pragma unroll 1` (one copy of the code, see swap_row_halves), the conversion loops over its load batches,
+// and linear mode is a separate instantiation.  tests/test_kernel_footprint.py holds k_edge_layer_wg2 to its budget.
 // ----------------------------------------------------------------------------------------------
-// TIMED adds the phase timers (clock reads pin instruction order, so the product entry points are built without).
-template <int NWG, bool TIMED = false>
+// LIN selects linear mode (k_linear_wg2); TIMED adds the phase timers (clock reads pin instruction order, so the product
+// entry points are built without).
+template <int NWG, bool LIN, bool TIMED = false>
 __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, const TcParams& P) {
   using Cfg = TcCfg<NWG>;
   constexpr int NSTAGE = Cfg::NSTAGE;
@@ -264,7 +283,7 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
   uint64_t* empty = full + NSTAGE;                                      // [NSTAGE] every consumer warp -> producer
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const bool lin = P.lin_out != nullptr;
+  constexpr bool lin = LIN;
   const int loads_per_tile = P.write_e ? 16 : 8;   // (C | O) x 4 K-chunks x (hi, lo)
 
   if (threadIdx.x == 0) {
@@ -406,7 +425,7 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
 
     // ---------------- GEMM1 A operand: fp32 rows -> bf16 hi/lo, K-major 128B-swizzled chunks ----------------
     // CONV_BATCH row loads of a thread are issued before the first split: one memory round trip per batch.
-#pragma unroll
+#pragma unroll 1
     for (int it0 = 0; it0 < 32; it0 += CONV_BATCH) {
       float4 x[CONV_BATCH];
 #pragma unroll
@@ -456,31 +475,30 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
     }
 
     // ---------------- E1: e_hat = acc + A h[col] + B h[row];  messages sigmoid(e_hat) * V h[col] ----------------
+    // E1 and E2 / E3 run once per row half h (rows lr0, lr0 + 8) on acc[4 j], acc[4 j + 1], then swap the halves.
     const float* src_a = w_src[lr0];
     const float* src_b = w_src[lr0 + 8];
-    {
-      const float* col_a = P.uvab + (size_t)(va ? P.g.col[sa] : 0) * 4 * H;
-      const float* col_b = P.uvab + (size_t)(vb ? P.g.col[sb] : 0) * 4 * H;
-      const float* row_a = P.uvab + (size_t)(va ? P.g.row[sa] : 0) * 4 * H + 3 * H;
-      const float* row_b = P.uvab + (size_t)(vb ? P.g.row[sb] : 0) * 4 * H + 3 * H;
+#pragma unroll 1
+    for (int h = 0; h < 2; ++h) {
+      const int s = h ? sb : sa;
+      const bool v = h ? vb : va;
+      const float* cp = P.uvab + (size_t)(v ? P.g.col[s] : 0) * 4 * H;
+      const float* rp = P.uvab + (size_t)(v ? P.g.row[s] : 0) * 4 * H + 3 * H;
+      const int r = lr0 + 8 * h;
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         const int c = 8 * j + 2 * t4;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const float* cp = h ? col_b : col_a;
-          const float2 ah = __ldg(reinterpret_cast<const float2*>(cp + 2 * H + c));
-          const float2 vh = __ldg(reinterpret_cast<const float2*>(cp + H + c));
-          const float2 bh = __ldg(reinterpret_cast<const float2*>((h ? row_b : row_a) + c));
-          const float x0 = (acc[4 * j + 2 * h] + ah.x) + bh.x;
-          const float x1 = (acc[4 * j + 2 * h + 1] + ah.y) + bh.y;
-          acc[4 * j + 2 * h] = x0;
-          acc[4 * j + 2 * h + 1] = x1;
-          const int r = lr0 + 8 * h;
-          *reinterpret_cast<float2*>(msg + r * H + (c ^ (8 * (r & 7)))) =
-              make_float2(sigmoid_mufu(x0) * vh.x, sigmoid_mufu(x1) * vh.y);
-        }
+        const float2 ah = __ldg(reinterpret_cast<const float2*>(cp + 2 * H + c));
+        const float2 vh = __ldg(reinterpret_cast<const float2*>(cp + H + c));
+        const float2 bh = __ldg(reinterpret_cast<const float2*>(rp + c));
+        const float x0 = (acc[4 * j] + ah.x) + bh.x;
+        const float x1 = (acc[4 * j + 1] + ah.y) + bh.y;
+        acc[4 * j] = x0;
+        acc[4 * j + 1] = x1;
+        *reinterpret_cast<float2*>(msg + r * H + (c ^ (8 * (r & 7)))) =
+            make_float2(sigmoid_mufu(x0) * vh.x, sigmoid_mufu(x1) * vh.y);
       }
+      swap_row_halves(acc);
     }
     wg_bar();   // messages of all 64 rows are in shared memory
     mark(PH_E1);
@@ -488,8 +506,8 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
     // ballot over the row table marks the rows that end a (group, node) segment: the next row has another node, or is
     // the group's last row, or lies past the last edge.  Rows past the last edge end no segment, so what they add to
     // `run` is never stored.  The row walk then has no per-row row-table loads and no early exit, and its one branch
-    // (store the sum at a marked row) is warp-uniform.  The loops stay rolled: the kernel's code does not fit the
-    // instruction cache, and unrolling them slowed every phase.
+    // (store the sum at a marked row) is warp-uniform.  The loops stay rolled: the kernel is bound by instruction fetch
+    // once its code grows, and unrolling them slowed every phase.
     const bool amax = P.agg_mode == AGG_MAX;
     const float run0 = amax ? -INFINITY : 0.0f;
 #pragma unroll 1
@@ -522,16 +540,16 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
     if (!P.write_e) continue;   // MIS last layer: the edge stream is never read again (gnn_encoder.py:412)
 
     // ---------------- E2 / E3: e_til = relu(LN_e(e_hat)) + tau;  s = silu(LN_O(e_til)) -> GEMM2 A operand ----------------
-#pragma unroll
+#pragma unroll 1
     for (int h = 0; h < 2; ++h) {
       float sum = 0.f;
 #pragma unroll
-      for (int j = 0; j < 32; ++j) sum += acc[4 * j + 2 * h] + acc[4 * j + 2 * h + 1];
+      for (int j = 0; j < 32; ++j) sum += acc[4 * j] + acc[4 * j + 1];
       float mean = quad_sum(sum) * (1.0f / H);
       float q = 0.f;
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
-        const float d0 = acc[4 * j + 2 * h] - mean, d1 = acc[4 * j + 2 * h + 1] - mean;
+        const float d0 = acc[4 * j] - mean, d1 = acc[4 * j + 1] - mean;
         q = fmaf(d0, d0, fmaf(d1, d1, q));
       }
       float rstd = rsqrtf(quad_sum(q) * (1.0f / H) + LN_EPS);
@@ -542,17 +560,17 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
         const float2 g = *reinterpret_cast<const float2*>(prm + c);
         const float2 b = *reinterpret_cast<const float2*>(prm + H + c);
         const float2 t = *reinterpret_cast<const float2*>(prm + 2 * H + c);
-        const float y0 = fmaxf(fmaf((acc[4 * j + 2 * h] - mean) * rstd, g.x, b.x), 0.0f) + t.x;
-        const float y1 = fmaxf(fmaf((acc[4 * j + 2 * h + 1] - mean) * rstd, g.y, b.y), 0.0f) + t.y;
-        acc[4 * j + 2 * h] = y0;
-        acc[4 * j + 2 * h + 1] = y1;
+        const float y0 = fmaxf(fmaf((acc[4 * j] - mean) * rstd, g.x, b.x), 0.0f) + t.x;
+        const float y1 = fmaxf(fmaf((acc[4 * j + 1] - mean) * rstd, g.y, b.y), 0.0f) + t.y;
+        acc[4 * j] = y0;
+        acc[4 * j + 1] = y1;
         sum += y0 + y1;
       }
       mean = quad_sum(sum) * (1.0f / H);
       q = 0.f;
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
-        const float d0 = acc[4 * j + 2 * h] - mean, d1 = acc[4 * j + 2 * h + 1] - mean;
+        const float d0 = acc[4 * j] - mean, d1 = acc[4 * j + 1] - mean;
         q = fmaf(d0, d0, fmaf(d1, d1, q));
       }
       rstd = rsqrtf(quad_sum(q) * (1.0f / H) + LN_EPS);
@@ -562,14 +580,15 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
         const int c = 8 * j + 2 * t4;
         const float2 g = *reinterpret_cast<const float2*>(prm + 3 * H + c);
         const float2 b = *reinterpret_cast<const float2*>(prm + 4 * H + c);
-        const float z0 = fmaf((acc[4 * j + 2 * h] - mean) * rstd, g.x, b.x);
-        const float z1 = fmaf((acc[4 * j + 2 * h + 1] - mean) * rstd, g.y, b.y);
+        const float z0 = fmaf((acc[4 * j] - mean) * rstd, g.x, b.x);
+        const float z1 = fmaf((acc[4 * j + 1] - mean) * rstd, g.y, b.y);
         uint32_t hi, lo;
         split2(z0 * sigmoid_mufu(z0), z1 * sigmoid_mufu(z1), hi, lo);   // SiLU
         const uint32_t off = (j >> 3) * 2 * TC_A_CHUNK + sw128_off(r, j & 7) + 4 * t4;
         *reinterpret_cast<uint32_t*>(a_reg + off) = hi;
         *reinterpret_cast<uint32_t*>(a_reg + off + TC_A_CHUNK) = lo;
       }
+      swap_row_halves(acc);
     }
     fence_proxy_async();
     wg_bar();
@@ -577,6 +596,8 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
     gemm(PH_G2_WAIT, PH_G2_MMA);   // GEMM2: acc = s * O^T
 
     // ---------------- E4: e = e_in + O(s) + b_O (in place) ----------------
+    // Both row halves stay unrolled here: as a rolled loop over h (swapping or shifting the halves), ptxas fails to
+    // allocate registers for the kernel at 232 per thread.
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       if (!(h ? vb : va)) continue;
@@ -607,22 +628,22 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
 // (64-row tiles, a different tiling of the same graph) is the A/B and validation variant (DFB_EDGE_IMPL_TC1).
 __global__ void __launch_bounds__(TcCfg<2>::THREADS, 1)
 k_edge_layer_wg2(const __grid_constant__ CUtensorMap wmap, const TcParams P) {
-  edge_layer_wg_body<2>(wmap, P);
+  edge_layer_wg_body<2, false>(wmap, P);
 }
 // the product kernel with phase timers (dfb_set_phase_timing): same results, read back by dfb_debug_phase_cycles
 __global__ void __launch_bounds__(TcCfg<2>::THREADS, 1)
 k_edge_layer_wg2_timed(const __grid_constant__ CUtensorMap wmap, const TcParams P) {
-  edge_layer_wg_body<2, true>(wmap, P);
+  edge_layer_wg_body<2, false, true>(wmap, P);
 }
 __global__ void __launch_bounds__(TcCfg<1>::THREADS, 1)
 k_edge_layer_wg1(const __grid_constant__ CUtensorMap wmap, const TcParams P) {
-  edge_layer_wg_body<1>(wmap, P);
+  edge_layer_wg_body<1, false>(wmap, P);
 }
 // the same body in linear mode (node-side / embedding linears) under its own name, so launch lists and profiles
-// do not mix the two uses
+// do not mix the two uses; the edge kernels carry none of its code
 __global__ void __launch_bounds__(TcCfg<2>::THREADS, 1)
 k_linear_wg2(const __grid_constant__ CUtensorMap wmap, const TcParams P) {
-  edge_layer_wg_body<2>(wmap, P);
+  edge_layer_wg_body<2, true>(wmap, P);
 }
 
 // ----------------------------------------------------------------------------------------------

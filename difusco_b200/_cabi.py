@@ -18,7 +18,7 @@ SYMBOLS = [
     "dfb_abi_version", "dfb_create", "dfb_destroy", "dfb_last_error", "dfb_set_aggregation",
     "dfb_set_edge_impl", "dfb_load_weights", "dfb_prepare_graph", "dfb_set_points",
     "dfb_encoder_forward", "dfb_denoise_step", "dfb_denoise", "dfb_denoise_host",
-    "dfb_launch_count", "dfb_profile_begin", "dfb_profile_end", "dfb_debug_edge_gemm",
+    "dfb_launch_count", "dfb_profile_begin", "dfb_profile_end", "dfb_debug_edge_gemm", "dfb_debug_gnn_layer",
     "dfb_debug_phase_cycles", "dfb_debug_watchdog", "dfb_knn_graph", "dfb_set_graph_capture",
     "dfb_set_phase_timing", "dfb_tsp_merge_sparse", "dfb_tsp_merge_order", "dfb_two_opt", "dfb_write_heatmap_txt",
 ]
@@ -58,6 +58,7 @@ def lib():
   L.dfb_profile_begin.argtypes = [vp]
   L.dfb_profile_end.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(i64)]
   L.dfb_debug_edge_gemm.argtypes = [vp, i32, vp, vp, vp]
+  L.dfb_debug_gnn_layer.argtypes = [vp, i32, f32, vp, vp, vp]
   L.dfb_debug_phase_cycles.argtypes = [vp, C.POINTER(C.c_uint64)]
   L.dfb_debug_watchdog.argtypes = [vp, C.POINTER(C.c_int)]
   L.dfb_set_graph_capture.argtypes = [vp, i32]
@@ -280,3 +281,8 @@ class Context(object):
 
   def debug_edge_gemm(self, layer, e_in_ptr, acc_out_ptr, stream=0):
     self._ck(lib().dfb_debug_edge_gemm(self._h, layer, e_in_ptr, acc_out_ptr, stream))
+
+  def debug_gnn_layer(self, layer, t, h_ptr, e_ptr, stream=0):
+    """Run GNN layer `layer` alone at timestep t, in place on device h (V,256) and e (E,256); e rows in the prepared
+    graph's stable row-sorted order."""
+    self._ck(lib().dfb_debug_gnn_layer(self._h, int(layer), float(t), h_ptr, e_ptr, stream))

@@ -48,7 +48,6 @@ struct dfb_ctx {
   const float *Wt_node = nullptr, *b_node = nullptr, *Wt_edge = nullptr, *b_edge = nullptr;
   const float *dimt128 = nullptr, *dimt256 = nullptr;
   float* lut = nullptr;   // [2][256] categorical edge-embedding LUT (inside wbuf)
-  float* cl0 = nullptr;   // [2][256] C_0 * lut (layer 0's GEMM1 by table lookup); followed by [2][256] zeros for the MIS e0 = 0 case
   // ---- graph ----
   bool graph_ready = false, points_ready = false;
   GraphDev g{};
@@ -385,7 +384,7 @@ extern "C" int dfb_load_weights(dfb_ctx* ctx, int n_layers, int hidden_dim, int 
 
   // frequency tables: computed by the Python host with the reference's own torch expressions and
   // passed as pseudo-tensors when available (bit-identical tables); otherwise computed here.
-  size_t o_freqs = put(TE), o_d128 = put(TE), o_d256 = put(H), o_lut = put(2 * H), o_cl0 = put(4 * H);
+  size_t o_freqs = put(TE), o_d128 = put(TE), o_d256 = put(H), o_lut = put(2 * H);
   auto it = sd.find("__const.time_freqs");
   for (int m = 0; m < TE; ++m)
     arena[o_freqs + m] = (it != sd.end() && it->second.second == TE)
@@ -427,7 +426,6 @@ extern "C" int dfb_load_weights(dfb_ctx* ctx, int n_layers, int hidden_dim, int 
   ctx->hp.out_channels = out_channels;
   ctx->dimt128 = base + o_d128; ctx->dimt256 = base + o_d256;
   ctx->lut = (float*)ctx->wbuf.p + o_lut;
-  ctx->cl0 = (float*)ctx->wbuf.p + o_cl0;   // second half stays zero (arena slots are zero-initialised)
   ctx->L = L; ctx->out_channels = out_channels; ctx->node_only = node_feature_only;
 
   int r = tc_bind_weights(&ctx->tc, (const uint16_t*)ctx->wbuf16.p, L);
@@ -442,9 +440,6 @@ extern "C" int dfb_load_weights(dfb_ctx* ctx, int n_layers, int hidden_dim, int 
     k_scalar_features<<<2, H>>>((const float*)ctx->tvals.p, nullptr, ctx->dimt256, (float*)ctx->feat.p, 2);
     CKL(ctx);
     k_linear<<<dim3(1, 1), 256>>>((const float*)ctx->feat.p, ctx->Wt_edge, ctx->b_edge, ctx->lut, 2, H);
-    CKL(ctx);
-    // layer 0 never needs its GEMM1: C_0 applied to the two possible input rows (fp32 FFMA; b_C rides in B h's bias)
-    k_linear<<<dim3(1, 1), 256>>>(ctx->lut, ctx->layers[0].Wt_C, nullptr, ctx->cl0, 2, H);
     CKL(ctx);
     CK(ctx, cudaDeviceSynchronize());
   }
@@ -639,7 +634,7 @@ extern "C" int dfb_set_points(dfb_ctx* ctx, const float* points, void* stream_) 
 // ================================================================================================
 // one forward (+ optional fused posterior)
 // ================================================================================================
-static int launch_edge_layer(dfb_ctx* ctx, int l, const float* uvab, const float* tvec_edge, int write_e,
+static int launch_edge_layer(dfb_ctx* ctx, int l, float* e, const float* uvab, const float* tvec_edge, int write_e,
                              int e_zero, const float* xt_for_lut, cudaStream_t st) {
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   if (ctx->profiling) {
@@ -656,17 +651,17 @@ static int launch_edge_layer(dfb_ctx* ctx, int l, const float* uvab, const float
   }
   const EdgeImpl impl = edge_impl(ctx);
   if (impl.fp32) {
-    if (e_zero) CK(ctx, cudaMemsetAsync(ctx->e.p, 0, (size_t)ctx->g.E * H * sizeof(float), st));
+    if (e_zero) CK(ctx, cudaMemsetAsync(e, 0, (size_t)ctx->g.E * H * sizeof(float), st));
     if (xt_for_lut) {
-      k_lut_expand<<<(ctx->g.E + 3) / 4, 256, 0, st>>>(xt_for_lut, ctx->g.perm, ctx->lut, (float*)ctx->e.p, ctx->g.E);
+      k_lut_expand<<<(ctx->g.E + 3) / 4, 256, 0, st>>>(xt_for_lut, ctx->g.perm, ctx->lut, e, ctx->g.E);
       CKL(ctx);
     }
-    k_edge_layer_fp32<<<ctx->g.n_groups, 256, EF_SMEM, st>>>((float*)ctx->e.p, uvab, (float*)ctx->partials.p,
+    k_edge_layer_fp32<<<ctx->g.n_groups, 256, EF_SMEM, st>>>(e, uvab, (float*)ctx->partials.p,
                                                             ctx->g, ctx->layers[l], tvec_edge, write_e,
                                                             ctx->agg_mode);
     CKL(ctx);
   } else {
-    if (tc_launch_edge_layer(&ctx->tc, l, (float*)ctx->e.p, uvab, (float*)ctx->partials.p, ctx->g, ctx->layers[l],
+    if (tc_launch_edge_layer(&ctx->tc, l, e, uvab, (float*)ctx->partials.p, ctx->g, ctx->layers[l],
                              tvec_edge, write_e, e_zero, xt_for_lut, ctx->lut, ctx->agg_mode, impl.nwg,
                              ctx->phase_timing, nullptr, st))
       FAIL(ctx, DFB_E_CUDA, "tensor-core edge layer: %s", ctx->tc.err.c_str());
@@ -676,14 +671,40 @@ static int launch_edge_layer(dfb_ctx* ctx, int l, const float* uvab, const float
   return DFB_OK;
 }
 
+// GNN layer l of the loaded model on the prepared graph, in place on h (V,256) and e (E,256, row-sorted), as
+// gnn_encoder.py:442-449 runs it: the node linears of h, the fused edge layer, then the node update.  tv is the layer's
+// time vector (on edges for TSP, on nodes for MIS).  Layer 0 of a forward passes its step-invariant inputs: uv0, TSP's
+// node linears of h0 (dfb_set_points), instead of computing them; e_zero (MIS: e0 = 0) or xt_lut (categorical TSP:
+// e0 read from the 2-row LUT) instead of reading e.  The last TSP layer skips the node update (TSP never reads h
+// after it, gnn_encoder.py:400) and the last MIS layer does not write e (gnn_encoder.py:412).
+static int run_layer(dfb_ctx* ctx, int l, float* h, float* e, const float* uv0, const float* tv, int e_zero,
+                     const float* xt_lut, cudaStream_t st) {
+  const int L = ctx->L;
+  const float* uv = uv0;
+  if (!uv) {
+    int r = node_linears(ctx, l, h, (float*)ctx->uvab.p, ctx->g.V, st);
+    if (r) return r;
+    uv = (const float*)ctx->uvab.p;
+  }
+  const int write_e = !(ctx->node_only && l == L - 1);
+  int r = launch_edge_layer(ctx, l, e, uv, ctx->node_only ? nullptr : tv, write_e, e_zero, xt_lut, st);
+  if (r) return r;
+  if (ctx->node_only || l < L - 1) {
+    k_node_update<<<(ctx->g.V + 7) / 8, 256, 0, st>>>(h, uv, (const float*)ctx->partials.p, ctx->g,
+                                                      ctx->layers[l].ln_h_g, ctx->layers[l].ln_h_b,
+                                                      ctx->node_only ? tv : nullptr, ctx->agg_mode);
+    CKL(ctx);
+  }
+  return DFB_OK;
+}
+
 // tvec: [L][256] for this step.  binary_xt: xt in {0,1} guaranteed (categorical denoise state).
 static int run_forward(dfb_ctx* ctx, const float* xt, const float* tvec, bool binary_xt, PosteriorArgs pa,
                        cudaStream_t st) {
   const GraphDev& g = ctx->g;
-  const int V = g.V, E = g.E, L = ctx->L;
+  const int V = g.V, E = g.E;
   float* h = (float*)ctx->h.p;
   float* e = (float*)ctx->e.p;
-  float* uvab = (float*)ctx->uvab.p;
   const float* xt_lut = nullptr;
   int e_zero = 0;
   if (!ctx->node_only) {
@@ -714,24 +735,11 @@ static int run_forward(dfb_ctx* ctx, const float* xt, const float* tvec, bool bi
     }
     e_zero = 1;   // gnn_encoder.py:407: e0 = zeros
   }
-  for (int l = 0; l < L; ++l) {
-    const float* uv = uvab;
-    if (l == 0 && !ctx->node_only) {
-      uv = (const float*)ctx->uvab0.p;
-    } else {
-      int r = node_linears(ctx, l, h, uvab, V, st);
-      if (r) return r;
-    }
-    const float* tv = tvec + (size_t)l * H;
-    int write_e = !(ctx->node_only && l == L - 1);
-    int r = launch_edge_layer(ctx, l, uv, ctx->node_only ? nullptr : tv, write_e, (l == 0) ? e_zero : 0,
-                              (l == 0) ? xt_lut : nullptr, st);
+  for (int l = 0; l < ctx->L; ++l) {
+    const bool first = l == 0;
+    int r = run_layer(ctx, l, h, e, (first && !ctx->node_only) ? (const float*)ctx->uvab0.p : nullptr,
+                      tvec + (size_t)l * H, first ? e_zero : 0, first ? xt_lut : nullptr, st);
     if (r) return r;
-    if (ctx->node_only || l < L - 1) {   // TSP never reads h after the last layer (gnn_encoder.py:400)
-      k_node_update<<<(V + 7) / 8, 256, 0, st>>>(h, uv, (const float*)ctx->partials.p, g, ctx->layers[l].ln_h_g,
-                                                 ctx->layers[l].ln_h_b, ctx->node_only ? tv : nullptr, ctx->agg_mode);
-      CKL(ctx);
-    }
   }
   // head
   const float* Z = ctx->node_only ? h : e;
@@ -1000,6 +1008,26 @@ extern "C" int dfb_debug_edge_gemm(dfb_ctx* ctx, int layer, const float* e_in, f
     FAIL(ctx, DFB_E_CUDA, "tensor-core edge layer: %s", ctx->tc.err.c_str());
   ctx->launches++;
   return DFB_OK;
+}
+
+// Test hook: GNN layer `layer` alone (run_layer, the code run_forward runs for it) at timestep t, in place on the
+// caller's h (V,256) and e (E,256, row-sorted).  Always reads e and computes the node linears of h: never the LUT,
+// e_zero or the cached layer-0 node linears.
+extern "C" int dfb_debug_gnn_layer(dfb_ctx* ctx, int layer, float t, float* h, float* e, void* stream_) {
+  if (!ctx) return DFB_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream_;
+  CK(ctx, cudaSetDevice(ctx->device));
+  if (!ctx->graph_ready) FAIL(ctx, DFB_E_INVALID, "dfb_prepare_graph must be called first");
+  if (layer < 0 || layer >= ctx->L) FAIL(ctx, DFB_E_INVALID, "layer %d out of range for %d layers", layer, ctx->L);
+  if (!is_device_ptr(h) || !is_device_ptr(e)) FAIL(ctx, DFB_E_INVALID, "h and e must be device pointers");
+  int slot;
+  int r = stage_acquire(ctx, &slot);
+  if (r) return r;
+  ctx->h_tvals[slot][0] = t;
+  r = compute_tvecs(ctx, slot, 1, st);
+  if (r) return r;
+  CK(ctx, cudaEventRecord(ctx->stage_ev[slot], st));
+  return run_layer(ctx, layer, h, e, nullptr, (const float*)ctx->tvec.p + (size_t)layer * H, 0, nullptr, st);
 }
 
 // Test/tuning hook: read and reset the per-phase cycle counters of the edge kernel (slots PH_* of edge_layer_tc.cuh).

@@ -176,6 +176,14 @@ int dfb_profile_end(dfb_ctx* ctx, double* edge_kernel_ms, int64_t* edge_kernel_l
  * acc_out (E,256).  DEVICE pointers.  Used by the parity tests to localise failures. */
 int dfb_debug_edge_gemm(dfb_ctx* ctx, int layer, const float* e_in, float* acc_out, void* stream);
 
+/* Test hook: GNN layer `layer` (0 <= layer < n_layers) of the loaded model alone, on the prepared graph, with the time
+ * vector of timestep t, in place on DEVICE buffers h (V,256) fp32 and e (E,256) fp32.  e is in the prepared graph's
+ * internal row-sorted order: the stable sort of edge_index[0] by dfb_prepare_graph (numpy: argsort(row, kind="stable")).
+ * Runs what a forward runs for that layer (node linears, fused edge layer, node update) with the selected edge impl and
+ * aggregation: the time vector goes to e (TSP) or h (MIS); after the last TSP layer h is left unchanged, after the last
+ * MIS layer e is.  Always reads e and h: never the categorical LUT, the MIS e0 = 0 or the cached layer-0 linears. */
+int dfb_debug_gnn_layer(dfb_ctx* ctx, int layer, float t, float* h, float* e, void* stream);
+
 /* Tuning hook: per-phase cycle counters of the edge kernel; out must hold 32 unsigned 64-bit values (host).  Only the
  * timed product kernel records them (dfb_set_phase_timing); otherwise the values read back as zero.  Read-and-reset.
  * Slots, each summed over every consumer warpgroup of every launch (SM clock cycles):

@@ -174,22 +174,29 @@ def _layer_sparse(w, l, h, e, row, col, V, aggregation="sum", gather_then_gemm=T
   return h_new, e_new                      # mode == "direct": no inner residual (:138)
 
 
+def layer_step(w, l, h, e, row, col, temb, time_on_edge, aggregation="sum", gather_then_gemm=True):
+  """Layer l of the encoder loop, gnn_encoder.py:442-449: the GNN layer, its time vector (on e for TSP, on h for
+  MIS), the residual on h and per_layer_out on e.  h (V,H), e (E,H) in the caller's edge order -> (h, e)."""
+  V, H = h.shape
+  h_in, e_in = h, e
+  h, e = _layer_sparse(w, l, h_in, e_in, row, col, V, aggregation, gather_then_gemm)
+  tv = w.lin(f"time_embed_layers.{l}.1", F.relu(temb))              # :329-337
+  if time_on_edge:
+    e = e + tv                                                       # :445
+  else:
+    h = h + tv                                                       # :447
+  h = h_in + h                                                       # :448
+  o = f"per_layer_out.{l}."
+  s = F.silu(F.layer_norm(e, (H,), w.t[o + "0.weight"], w.t[o + "0.bias"]))
+  e = e_in + w.lin(o + "2", s)                                       # :449
+  return h, e
+
+
 def _sparse_encoding(w, h, e, row, col, temb, time_on_edge, aggregation="sum", taps=None,
                      gather_then_gemm=True):
   """gnn_encoder.py:416-450 (non-checkpointed branch :442-449)."""
-  V, H = h.shape
   for l in range(w.n_layers):
-    h_in, e_in = h, e
-    h, e = _layer_sparse(w, l, h_in, e_in, row, col, V, aggregation, gather_then_gemm)
-    tv = w.lin(f"time_embed_layers.{l}.1", F.relu(temb))            # :329-337
-    if time_on_edge:
-      e = e + tv                                                     # :445
-    else:
-      h = h + tv                                                     # :447
-    h = h_in + h                                                     # :448
-    o = f"per_layer_out.{l}."
-    s = F.silu(F.layer_norm(e, (H,), w.t[o + "0.weight"], w.t[o + "0.bias"]))
-    e = e_in + w.lin(o + "2", s)                                     # :449
+    h, e = layer_step(w, l, h, e, row, col, temb, time_on_edge, aggregation, gather_then_gemm)
     if taps is not None:
       taps.append((h, e))
   return h, e

@@ -149,3 +149,72 @@ def regime(name, weights, fwd, node_head, seed=0):
   else:
     raise ValueError(name)
   return w
+
+
+# ------------------------------------------------------------------------------------------------
+# Irregular graphs: (V, edge_index (2,E) int64), rows sorted; deterministic from fixed seeds
+# ------------------------------------------------------------------------------------------------
+def graph_from_degrees(deg, rng, cols=None):
+  deg = np.asarray(deg, np.int64)
+  V = deg.size
+  rows = np.repeat(np.arange(V, dtype=np.int64), deg)
+  if cols is None:
+    cols = rng.integers(0, V, rows.size)
+  return V, np.stack([rows, np.asarray(cols, np.int64)])
+
+
+def hub_graph():
+  """Node 500 has degree 3000 (edges 500..3499: 24 tiles of 128 rows, 94 groups); the other 1200 nodes are
+  degree-1 leaves pointing at the hub, so each of the groups before and after it holds 32 distinct nodes."""
+  rng = np.random.default_rng(11)
+  V, hub = 1201, 500
+  deg = np.ones(V, np.int64)
+  deg[hub] = 3000
+  rows = np.repeat(np.arange(V), deg)
+  cols = np.where(rows == hub, rng.integers(0, V, rows.size), hub)
+  return graph_from_degrees(deg, rng, cols)
+
+
+ISOLATED = [0, 1, 2, 60, 61, 62, 63, 64, 130, 132, 134, 234, 235, 236, 237, 238, 239]
+
+
+def isolated_graph():
+  """Nodes without edges at the start, as a run and singly between nodes that share a 32-edge group, and at the
+  end of the index range (the caller passes points / xt for them too)."""
+  rng = np.random.default_rng(12)
+  deg = rng.integers(1, 5, 240)
+  deg[ISOLATED] = 0
+  return graph_from_degrees(deg, rng)
+
+
+# cumulative ends land on, one before and one after multiples of 32, 64 and 128 (test_gpu_graph_edges.py checks it)
+DEGREES = [31, 1, 32, 33, 31, 1, 63, 65, 127, 1, 128, 129, 127, 64, 64, 1, 31, 33, 2, 62, 65, 63, 129, 128, 124, 1,
+           63, 1, 127, 129]
+
+
+def degseq_graph():
+  return graph_from_degrees(DEGREES, np.random.default_rng(13))
+
+
+def dup_graph():
+  """A ring without self loops in which every edge appears one to three times."""
+  rng = np.random.default_rng(14)
+  V = 150
+  r, c = [], []
+  for i in range(V):
+    for j in ((i + 1) % V, (i - 1) % V):
+      k = int(rng.integers(1, 4))
+      r += [i] * k
+      c += [j] * k
+  return V, np.array([r, c], np.int64)
+
+
+TINY = {1: 1, 2: 2, 31: 3, 33: 4, 63: 9, 65: 5, 127: 7, 129: 9}   # E -> V
+
+
+def tiny_graph(E):
+  """E < 129 edges on at most 9 nodes: one partial tile, the second warpgroup idle for E < 64, duplicates."""
+  rng = np.random.default_rng(100 + E)
+  V = TINY[E]
+  rows = np.sort(rng.integers(0, V, E))
+  return V, np.stack([rows, rng.integers(0, V, E)]).astype(np.int64)

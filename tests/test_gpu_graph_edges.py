@@ -24,77 +24,8 @@ TOL = 1e-4
 T_FWD = 700.0
 
 
-# ------------------------------------------------------------------------------------------------
-# graph generators: (V, edge_index (2,E) int64, rows sorted unless shuffled)
-# ------------------------------------------------------------------------------------------------
-def _graph_from_degrees(deg, rng, cols=None):
-  deg = np.asarray(deg, np.int64)
-  V = deg.size
-  rows = np.repeat(np.arange(V, dtype=np.int64), deg)
-  if cols is None:
-    cols = rng.integers(0, V, rows.size)
-  return V, np.stack([rows, np.asarray(cols, np.int64)])
-
-
-def _hub():
-  """Node 500 has degree 3000 (edges 500..3499: 24 tiles of 128 rows, 94 groups); the other 1200 nodes are
-  degree-1 leaves pointing at the hub, so each of the groups before and after it holds 32 distinct nodes."""
-  rng = np.random.default_rng(11)
-  V, hub = 1201, 500
-  deg = np.ones(V, np.int64)
-  deg[hub] = 3000
-  rows = np.repeat(np.arange(V), deg)
-  cols = np.where(rows == hub, rng.integers(0, V, rows.size), hub)
-  return _graph_from_degrees(deg, rng, cols)
-
-
-ISOLATED = [0, 1, 2, 60, 61, 62, 63, 64, 130, 132, 134, 234, 235, 236, 237, 238, 239]
-
-
-def _isolated():
-  """Nodes without edges at the start, as a run and singly between nodes that share a 32-edge group, and at the
-  end of the index range (the caller passes points / xt for them too)."""
-  rng = np.random.default_rng(12)
-  deg = rng.integers(1, 5, 240)
-  deg[ISOLATED] = 0
-  return _graph_from_degrees(deg, rng)
-
-
-# cumulative ends land on, one before and one after multiples of 32, 64 and 128 (checked in the test below)
-DEGREES = [31, 1, 32, 33, 31, 1, 63, 65, 127, 1, 128, 129, 127, 64, 64, 1, 31, 33, 2, 62, 65, 63, 129, 128, 124, 1,
-           63, 1, 127, 129]
-
-
-def _degseq():
-  return _graph_from_degrees(DEGREES, np.random.default_rng(13))
-
-
-def _dup():
-  """A ring without self loops in which every edge appears one to three times."""
-  rng = np.random.default_rng(14)
-  V = 150
-  r, c = [], []
-  for i in range(V):
-    for j in ((i + 1) % V, (i - 1) % V):
-      k = int(rng.integers(1, 4))
-      r += [i] * k
-      c += [j] * k
-  return V, np.array([r, c], np.int64)
-
-
-TINY = {1: 1, 2: 2, 31: 3, 33: 4, 63: 9, 65: 5, 127: 7, 129: 9}   # E -> V
-
-
-def _tiny(E):
-  """E < 129 edges on at most 9 nodes: one partial tile, the second warpgroup idle for E < 64, duplicates."""
-  rng = np.random.default_rng(100 + E)
-  V = TINY[E]
-  rows = np.sort(rng.integers(0, V, E))
-  return V, np.stack([rows, rng.integers(0, V, E)]).astype(np.int64)
-
-
-FAMILIES = {"hub": _hub, "isolated": _isolated, "degseq": _degseq, "dup": _dup}
-FAMILIES.update({f"tiny{E}": (lambda E=E: _tiny(E)) for E in TINY})
+FAMILIES = {"hub": G.hub_graph, "isolated": G.isolated_graph, "degseq": G.degseq_graph, "dup": G.dup_graph}
+FAMILIES.update({f"tiny{E}": (lambda E=E: G.tiny_graph(E)) for E in G.TINY})
 CASES = [f + s for f in FAMILIES for s in ("", "_shuf")]
 
 _case_cache = {}
@@ -155,19 +86,19 @@ def _ref64(weights2, case, task, agg):
 
 
 def test_generators_reach_the_boundaries_they_are_meant_to():
-  ends = np.cumsum(DEGREES)
+  ends = np.cumsum(G.DEGREES)
   for b in (32, 64, 128):
     assert {-1, 0, 1} <= {int(x) for x in ((ends + 1) % b) - 1}, b
-  V, ei = _hub()
+  V, ei = G.hub_graph()
   deg = np.bincount(ei[0], minlength=V)
   assert deg.max() == 3000 and (deg.max() + 127) // 128 > 20 and (np.sort(deg)[:-1] == 1).all()
-  V, ei = _isolated()
+  V, ei = G.isolated_graph()
   deg = np.bincount(ei[0], minlength=V)
-  assert set(np.flatnonzero(deg == 0)) == set(ISOLATED)
-  V, ei = _dup()
+  assert set(np.flatnonzero(deg == 0)) == set(G.ISOLATED)
+  V, ei = G.dup_graph()
   assert (ei[0] != ei[1]).all() and len({(a, b) for a, b in ei.T}) < ei.shape[1]
-  for E, V in TINY.items():
-    v, ei = _tiny(E)
+  for E, V in G.TINY.items():
+    v, ei = G.tiny_graph(E)
     assert ei.shape == (2, E) and v == V and ei.max() < V
   for c in CASES:
     ei = _case(c)[1]

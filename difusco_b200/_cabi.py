@@ -17,7 +17,7 @@ AGGREGATION = {"sum": 0, "mean": 1, "max": 2}
 SYMBOLS = [
     "dfb_abi_version", "dfb_create", "dfb_destroy", "dfb_last_error", "dfb_set_aggregation",
     "dfb_set_edge_impl", "dfb_load_weights", "dfb_prepare_graph", "dfb_set_points",
-    "dfb_encoder_forward", "dfb_denoise_step", "dfb_denoise", "dfb_denoise_host",
+    "dfb_encoder_forward", "dfb_denoise_step", "dfb_denoise", "dfb_denoise_record", "dfb_denoise_host",
     "dfb_launch_count", "dfb_profile_begin", "dfb_profile_end", "dfb_debug_edge_gemm", "dfb_debug_gnn_layer",
     "dfb_debug_phase_cycles", "dfb_debug_watchdog", "dfb_knn_graph", "dfb_set_graph_capture",
     "dfb_set_phase_timing", "dfb_tsp_merge_sparse", "dfb_tsp_merge_order", "dfb_two_opt", "dfb_write_heatmap_txt",
@@ -51,6 +51,8 @@ def lib():
   L.dfb_denoise_step.argtypes = [vp, i32, vp, f32, C.POINTER(f32), i32, vp, u64, i32, vp, vp, vp, vp]
   L.dfb_denoise.argtypes = [vp, i32, vp, i32, C.POINTER(C.c_int32), C.POINTER(f32),
                             C.POINTER(C.c_int32), vp, u64, vp]
+  L.dfb_denoise_record.argtypes = [vp, i32, vp, i32, C.POINTER(C.c_int32), C.POINTER(f32), C.POINTER(C.c_int32), vp,
+                                   u64, i32, C.POINTER(C.c_int32), vp, vp, vp, vp]
   L.dfb_denoise_host.argtypes = [vp, i32, vp, vp, i64, i64, i32, vp, i32, C.POINTER(C.c_int32),
                                  C.POINTER(f32), C.POINTER(C.c_int32), u64, vp, vp]
   L.dfb_launch_count.argtypes = [vp]
@@ -225,6 +227,17 @@ class Context(object):
     steps, t1a, ca, la = self._sched_arrays(t1, consts, last)
     self._ck(lib().dfb_denoise(self._h, diffusion, xt_ptr, steps, t1a, ca, la, uniforms_ptr,
                                int(seed) & 0xFFFFFFFFFFFFFFFF, stream))
+
+  def denoise_record(self, diffusion, xt_ptr, t1, consts, last, record_steps, rec_xt_ptr=None, rec_p_ptr=None,
+                     rec_out_ptr=None, uniforms_ptr=None, seed=0, stream=0):
+    """denoise that also writes, at each step record_steps[j], row j of the device buffers rec_xt (n_rec, N),
+    rec_p (n_rec, N) and rec_out (n_rec, N, out_channels); any of them may be None."""
+    steps, t1a, ca, la = self._sched_arrays(t1, consts, last)
+    n_rec = len(record_steps)
+    ra = (C.c_int32 * max(n_rec, 1))(*[int(x) for x in record_steps])
+    self._ck(lib().dfb_denoise_record(self._h, diffusion, xt_ptr, steps, t1a, ca, la, uniforms_ptr,
+                                      int(seed) & 0xFFFFFFFFFFFFFFFF, n_rec, ra, rec_xt_ptr, rec_p_ptr, rec_out_ptr,
+                                      stream))
 
   def denoise_host(self, diffusion, points_ptr, edge_index_ptr, num_nodes, num_edges, gn_segments, xt0_ptr,
                    t1, consts, last, seed, heatmap_ptr, stream=0):

@@ -853,6 +853,14 @@ static int enqueue_loop(dfb_ctx* ctx, int diffusion_type, float* xt, int steps, 
 extern "C" int dfb_denoise(dfb_ctx* ctx, int diffusion_type, float* xt, int steps, const int32_t* t1,
                            const float* consts, const int32_t* last_flags, const float* uniforms,
                            uint64_t seed, void* stream_) {
+  return dfb_denoise_record(ctx, diffusion_type, xt, steps, t1, consts, last_flags, uniforms, seed, 0, nullptr,
+                            nullptr, nullptr, nullptr, stream_);
+}
+
+extern "C" int dfb_denoise_record(dfb_ctx* ctx, int diffusion_type, float* xt, int steps, const int32_t* t1,
+                                  const float* consts, const int32_t* last_flags, const float* uniforms,
+                                  uint64_t seed, int n_record, const int32_t* record_steps, float* rec_xt,
+                                  float* rec_p, float* rec_out, void* stream_) {
   if (!ctx) return DFB_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream_;
   CK(ctx, cudaSetDevice(ctx->device));
@@ -864,16 +872,38 @@ extern "C" int dfb_denoise(dfb_ctx* ctx, int diffusion_type, float* xt, int step
     int r = step_args(ctx, diffusion_type, nullptr, 0, &chk);
     if (r) return r;
   }
+  if (n_record < 0) FAIL(ctx, DFB_E_INVALID, "n_record %d < 0", n_record);
+  if (n_record > 0) {
+    if (!record_steps) FAIL(ctx, DFB_E_INVALID, "n_record > 0 needs record_steps");
+    if (!rec_xt && !rec_p && !rec_out) FAIL(ctx, DFB_E_INVALID, "n_record > 0 with no record buffer");
+    if (rec_p && diffusion_type != DFB_DIFFUSION_CATEGORICAL)
+      FAIL(ctx, DFB_E_INVALID, "rec_p is the categorical posterior: not defined for gaussian diffusion");
+    for (int j = 0; j < n_record; ++j) {
+      if (record_steps[j] < 0 || record_steps[j] >= steps)
+        FAIL(ctx, DFB_E_INVALID, "record step %d outside [0, %d)", record_steps[j], steps);
+      if (j > 0 && record_steps[j] <= record_steps[j - 1])
+        FAIL(ctx, DFB_E_INVALID, "record steps must be strictly increasing (%d after %d)", record_steps[j],
+             record_steps[j - 1]);
+    }
+  }
   int slot;
   int r = stage_acquire(ctx, &slot);
   if (r) return r;
-  for (int i = 0; i < steps; ++i) {
+  const size_t N = ctx->node_only ? ctx->g.V : ctx->g.E;
+  for (int i = 0, j = 0; i < steps; ++i) {
     ctx->h_tvals[slot][i] = (float)t1[i];
     StepParams& sp = ctx->h_steps[slot][i];
     for (int k = 0; k < 4; ++k) sp.c[k] = consts[4 * i + k];
     sp.last = last_flags[i];
     sp.step = (unsigned)i;
     sp.seed = seed;
+    sp.rec_xt = sp.rec_p = sp.rec_out = nullptr;
+    if (j < n_record && record_steps[j] == i) {
+      if (rec_xt) sp.rec_xt = rec_xt + (size_t)j * N;
+      if (rec_p) sp.rec_p = rec_p + (size_t)j * N;
+      if (rec_out) sp.rec_out = rec_out + (size_t)j * N * ctx->out_channels;
+      ++j;
+    }
   }
   ENS(ctx, ctx->d_steps, (size_t)dfb_ctx::MAX_STEPS * sizeof(StepParams));
   r = compute_tvecs(ctx, slot, steps, st);
@@ -881,7 +911,6 @@ extern "C" int dfb_denoise(dfb_ctx* ctx, int diffusion_type, float* xt, int step
   CK(ctx, cudaMemcpyAsync(ctx->d_steps.p, ctx->h_steps[slot], (size_t)steps * sizeof(StepParams), cudaMemcpyHostToDevice, st));
   CK(ctx, cudaEventRecord(ctx->stage_ev[slot], st));
   // the loop state lives in the context's own buffer, so the captured graph does not depend on the caller's pointer
-  const size_t N = ctx->node_only ? ctx->g.V : ctx->g.E;
   float* x = (float*)ctx->d_xt.p;
   if (xt != x) CK(ctx, cudaMemcpyAsync(x, xt, N * sizeof(float), cudaMemcpyDeviceToDevice, st));
 

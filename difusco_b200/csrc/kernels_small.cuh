@@ -279,11 +279,16 @@ struct HeadParams {
 enum { HEAD_FORWARD = 0, HEAD_CATEGORICAL = 1, HEAD_GAUSSIAN = 2 };
 // Per-step posterior parameters in DEVICE memory: the captured CUDA graph of the denoise loop reads them through a
 // pointer, so one graph serves every schedule / seed of the same shape (only this small table is re-uploaded).
+// rec_*: this step's row of the caller's trajectory buffers (dfb_denoise_record), null when the step is not recorded;
+// living in the table, they do not make the graph depend on the caller's buffers either.
 struct StepParams {
   float c[4];
   int last;
   unsigned int step;
   unsigned long long seed;
+  float* rec_xt;    // (N,) state after the step
+  float* rec_p;     // (N,) categorical p before sampling
+  float* rec_out;   // (N, out_channels) network output
 };
 struct PosteriorArgs {
   int mode;            // HEAD_*
@@ -301,7 +306,7 @@ struct PosteriorArgs {
 __device__ __forceinline__ void head_posterior(const HeadParams& hp, const PosteriorArgs& pa_in, size_t o, float l0, float l1) {
   PosteriorArgs pa = pa_in;
   if (pa.sp) {
-    const StepParams sp = *pa.sp;
+    const StepParams& sp = *pa.sp;
     pa.c[0] = sp.c[0]; pa.c[1] = sp.c[1]; pa.c[2] = sp.c[2]; pa.c[3] = sp.c[3];
     pa.last = sp.last; pa.step = sp.step; pa.seed = sp.seed;
   }
@@ -309,15 +314,15 @@ __device__ __forceinline__ void head_posterior(const HeadParams& hp, const Poste
     pa.net_out[o * hp.out_channels] = l0;
     if (hp.out_channels == 2) pa.net_out[o * 2 + 1] = l1;
   }
+  float p = 0.0f, res = 0.0f;
   if (pa.mode == HEAD_CATEGORICAL) {
     float m = fmaxf(l0, l1);
     float e0 = expf(l0 - m), e1 = expf(l1 - m);
     float inv = 1.0f / (e0 + e1);
     float p0 = e0 * inv, p1 = e1 * inv;
     int x = pa.xt_in[o] != 0.0f;
-    float p = __fadd_rn(__fmul_rn(pa.c[2 * x], p0), __fmul_rn(pa.c[2 * x + 1], p1));
+    p = __fadd_rn(__fmul_rn(pa.c[2 * x], p0), __fmul_rn(pa.c[2 * x + 1], p1));
     if (pa.p_out) pa.p_out[o] = p;
-    float res;
     if (pa.last) {
       res = fmaxf(p, 0.0f);
     } else {
@@ -333,7 +338,19 @@ __device__ __forceinline__ void head_posterior(const HeadParams& hp, const Poste
       float zn = pa.uniforms ? pa.uniforms[o] : philox_normal(pa.seed, pa.step, o);
       y = fmaf(pa.c[3], zn, y);
     }
-    pa.xt_out[o] = y;
+    res = y;
+    pa.xt_out[o] = res;
+  }
+  // trajectory recording (dfb_denoise_record), last and through pa_in, the kernel parameter: the record pointers are
+  // then loaded only here, and k_head keeps the spills it had without them
+  if (pa_in.sp) {
+    const StepParams& sp = *pa_in.sp;
+    if (sp.rec_out) {
+      sp.rec_out[o * hp.out_channels] = l0;
+      if (hp.out_channels == 2) sp.rec_out[o * 2 + 1] = l1;
+    }
+    if (sp.rec_p) sp.rec_p[o] = p;
+    if (sp.rec_xt) sp.rec_xt[o] = res;
   }
 }
 

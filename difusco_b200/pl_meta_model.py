@@ -194,8 +194,13 @@ class COMetaModel(_Base):
                      torch.cuda.current_stream().cuda_stream)
     return (out, p) if want_prob else out
 
-  def _fused_loop(self, xt, steps, seed=None):
-    """The whole reverse-diffusion loop on device (pl_tsp_model.py:207-217).  In place on xt."""
+  def _fused_loop(self, xt, steps, seed=None, record_steps=None):
+    """The whole reverse-diffusion loop on device (pl_tsp_model.py:207-217).  In place on xt.
+
+    record_steps (a list of step indices, or "all") also records those steps from inside the same loop and returns
+    (xt, trace): trace["steps"] the recorded step indices, "t" their source timesteps t1, "xt" (n_rec, N) the state
+    after each step, "p" (n_rec, N) the categorical p before sampling (categorical only), "out" (n_rec, N,
+    out_channels) the network output; all CUDA tensors in xt's element order."""
     from .utils.diffusion_schedulers import InferenceSchedule
     ctx = self.model.engine()
     sched = InferenceSchedule(inference_schedule=self.args.inference_schedule, T=self.diffusion.T,
@@ -210,5 +215,22 @@ class COMetaModel(_Base):
     if seed is None:   # honour torch.manual_seed like the reference's torch.bernoulli would
       seed = int(torch.randint(0, 2 ** 62, (1,)).item())
     mode = _cabi.CATEGORICAL if self.diffusion_type == "categorical" else _cabi.GAUSSIAN
-    ctx.denoise(mode, xt.data_ptr(), t1s, consts, lasts, None, seed, torch.cuda.current_stream().cuda_stream)
-    return xt
+    stream = torch.cuda.current_stream().cuda_stream
+    if record_steps is None:
+      ctx.denoise(mode, xt.data_ptr(), t1s, consts, lasts, None, seed, stream)
+      return xt
+    rec = list(range(steps)) if isinstance(record_steps, str) and record_steps == "all" else \
+        [int(s) for s in record_steps]
+    if any(s < 0 or s >= steps for s in rec) or any(b <= a for a, b in zip(rec, rec[1:])):
+      raise ValueError(f"record_steps must be strictly increasing and inside [0, {steps}): {rec}")
+    n, dev = xt.numel(), xt.device
+    out_channels = 2 if mode == _cabi.CATEGORICAL else 1
+    trace = {"steps": torch.tensor(rec, dtype=torch.int64, device=dev),
+             "t": torch.tensor([t1s[s] for s in rec], dtype=torch.int64, device=dev),
+             "xt": torch.empty((len(rec), n), device=dev, dtype=torch.float32),
+             "out": torch.empty((len(rec), n, out_channels), device=dev, dtype=torch.float32)}
+    if mode == _cabi.CATEGORICAL:
+      trace["p"] = torch.empty((len(rec), n), device=dev, dtype=torch.float32)
+    ctx.denoise_record(mode, xt.data_ptr(), t1s, consts, lasts, rec, trace["xt"].data_ptr(),
+                       trace["p"].data_ptr() if "p" in trace else None, trace["out"].data_ptr(), None, seed, stream)
+    return xt, trace

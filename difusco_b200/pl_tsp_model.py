@@ -18,6 +18,16 @@ from .pl_meta_model import COMetaModel
 from .utils.tsp_utils import TSPEvaluator, batched_two_opt_torch, merge_tours
 
 
+def _shape_trace(trace, shape):
+  """The (n_rec, N[, out_channels]) record tensors reshaped to (n_rec, *shape[, out_channels])."""
+  out = dict(trace)
+  for k in ("xt", "p"):
+    if k in out:
+      out[k] = out[k].reshape((-1,) + tuple(shape))
+  out["out"] = out["out"].reshape((-1,) + tuple(shape) + (out["out"].shape[-1],))
+  return out
+
+
 class TSPModel(COMetaModel):
   def __init__(self, param_args=None):
     super().__init__(param_args=param_args, node_feature_only=False)
@@ -52,15 +62,22 @@ class TSPModel(COMetaModel):
     return self._denoise_step(points, xt, t, device, edge_index, target_t)
 
   # ------------------------------------------------------------------------------------
-  def denoise_heatmap(self, points, edge_index, xt, steps=None, seed=None):
-    """xt0 -> raw final xt on device, the whole loop fused (no host sync inside)."""
+  def denoise_heatmap(self, points, edge_index, xt, steps=None, seed=None, record_steps=None):
+    """xt0 -> raw final xt on device, the whole loop fused (no host sync inside).
+
+    record_steps (step indices or "all"): returns (heatmap, trace) instead, trace as COMetaModel._fused_loop with
+    each tensor shaped like xt after its leading step dimension: (n_rec, E) sparse, (n_rec, B, V, V) dense; "out"
+    has a trailing out_channels dimension."""
     steps = steps or self.args.inference_diffusion_steps
     with torch.no_grad():
       dev = self.model._device()
       self._prepare(points.to(dev), edge_index.to(dev) if edge_index is not None else None, dev)
       x = xt.reshape(-1).float().contiguous().to(dev).clone()
-      self._fused_loop(x, steps, seed)
-      return x.reshape(xt.shape)
+      if record_steps is None:
+        self._fused_loop(x, steps, seed)
+        return x.reshape(xt.shape)
+      _, trace = self._fused_loop(x, steps, seed, record_steps)
+      return x.reshape(xt.shape), _shape_trace(trace, xt.shape)
 
   # ------------------------------------------------------------------------------------
   # test_step = unpack -> (sample, fused denoise loop, decode) x sequential_sampling -> metrics

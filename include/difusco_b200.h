@@ -116,6 +116,22 @@ int dfb_denoise(dfb_ctx* ctx, int diffusion_type, float* xt, int steps, const in
                 const float* consts, const int32_t* last_flags, const float* uniforms,
                 uint64_t seed, void* stream);
 
+/* dfb_denoise that also records the trajectory: the same loop (dfb_denoise is this call with n_record = 0), and at
+ * each step record_steps[j] it writes, in the caller's element order, into row j of
+ *   rec_xt   DEVICE (n_record, N)               the state after the step: categorical the Bernoulli sample, at the
+ *                                               last step clamp(p, min=0) (the heatmap); gaussian the updated xt
+ *   rec_p    DEVICE (n_record, N)               categorical p before sampling (must be NULL for gaussian)
+ *   rec_out  DEVICE (n_record, N, out_channels) raw network output (logits / the gaussian prediction)
+ * Any buffer may be NULL (not recorded); at least one must be given when n_record > 0.  record_steps is HOST
+ * (n_record,), strictly increasing, every value in [0, steps).  The final xt is bitwise dfb_denoise's.  The record
+ * pointers travel in the per-step device table, so changing buffers or steps replays the same captured graph; rows
+ * are written from inside it.  Bad arguments return DFB_E_INVALID before any device work, writing nothing.
+ * Size: steps x N x (8 + 4 out_channels) bytes when every step and quantity is recorded. */
+int dfb_denoise_record(dfb_ctx* ctx, int diffusion_type, float* xt, int steps, const int32_t* t1,
+                       const float* consts, const int32_t* last_flags, const float* uniforms, uint64_t seed,
+                       int n_record, const int32_t* record_steps, float* rec_xt, float* rec_p, float* rec_out,
+                       void* stream);
+
 /* dfb_denoise replays the whole loop as ONE captured CUDA graph (on a stream of the library, fenced to `stream` by
  * events; re-captured only when the prepared graph, the buffers, the implementation switches or `steps` change).
  * dfb_set_graph_capture(ctx, 0) turns that off (plain launches).  Environment DFB_GRAPH_CAPTURE=0 does the same. */

@@ -12,8 +12,11 @@
 //                         LayerNorm epilogues straight out of the accumulator registers (a row lives in the 4 threads
 //                         of a quad), writes GEMM2's A operand over GEMM1's and finishes with the residual update.
 //   warpgroup NWG         TMA producer (one thread): streams the bf16 hi/lo weight K-chunks [256 rows x 64 K] (128B
-//                         swizzle) through an NSTAGE ring that every consumer warpgroup reads.  With two consumer
-//                         warpgroups it hands its registers to them (setmaxnreg 40 / 232): no spills in the epilogue.
+//                         swizzle) through an NSTAGE ring, each GEMM's 8 chunks once per consumer warpgroup.  With two
+//                         consumer warpgroups it hands its registers to them (setmaxnreg 40 / 232): no spills in the
+//                         epilogue.
+// Two consumer warpgroups take turns on the tensor cores (ping-pong): one runs a GEMM alone while the other runs an
+// epilogue, so each GEMM overlaps the other warpgroup's memory waits instead of sharing the tensor cores with its GEMM.
 // Per-(32-edge group, node) message sums go through shared memory (the dead GEMM1 operand) and are reduced in a fixed
 // order per column: deterministic, no atomics.
 // Precision: every 256x256 product is evaluated as  a_hi*b_hi + a_lo*b_hi + a_hi*b_lo  with
@@ -241,7 +244,8 @@ __device__ __forceinline__ void swap_row_halves(float (&d)[128]) {
 
 // Phase timers of the instrumented entry point k_edge_layer_wg2_timed: slots of TcParams::phase_cycles, summed over
 // every consumer warpgroup of the launch (SM clock cycles read by thread 0 of the warpgroup).  The phases partition the
-// tile loop, so their sum never exceeds PH_TOTAL.
+// tile loop, so their sum never exceeds PH_TOTAL; what PH_TOTAL holds beyond them is the time spent waiting for the
+// turn on the tensor cores, which has no slot of its own (slots past PH_E4 stay zero).
 enum {
   PH_TILES = 0,   // tiles processed (one count per warpgroup and tile)
   PH_TOTAL,       // cycles from the first tile to the end of the tile loop
@@ -280,16 +284,17 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
   int* s_row = reinterpret_cast<int*>(smem + Cfg::OFF_ROW);
   const float** s_src = reinterpret_cast<const float**>(smem + Cfg::OFF_SRC);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);   // [NSTAGE] TMA -> consumers (expect_tx)
-  uint64_t* empty = full + NSTAGE;                                      // [NSTAGE] every consumer warp -> producer
+  uint64_t* empty = full + NSTAGE;                                      // [NSTAGE] the 4 reading warps -> producer
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr bool lin = LIN;
-  const int loads_per_tile = P.write_e ? 16 : 8;   // (C | O) x 4 K-chunks x (hi, lo)
+  // (C | O) x consumer warpgroup x 4 K-chunks x (hi, lo): C for warpgroup 0, C for warpgroup 1, then O likewise
+  const int loads_per_tile = (P.write_e ? 16 : 8) * NWG;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < NSTAGE; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 4 * NWG);
+      mbar_init(&empty[s], 4);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     fence_proxy_async();
@@ -317,7 +322,7 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
           mbar_arrive_expect_tx(&full[s], TC_B_BYTES);
           // hi, lo of C, then of O; linear mode: hi, lo of block (tile & 3) of U|V|A|B, or of the one embedding
           const int row = (lin ? P.lin_w_row + (P.lin_nb == 4 ? (tile & 3) : 0) * W_MAT_ROWS
-                               : P.w_row_base + (i >= 8 ? w_row_O(0) - w_row_C(0) : 0)) +
+                               : P.w_row_base + (i >= 8 * NWG ? w_row_O(0) - w_row_C(0) : 0)) +
                           (i & 1) * W_LO_ROWS;
           tma_load_2d(smem_base + Cfg::OFF_B + s * TC_B_BYTES, &wmap, &full[s], ((i >> 1) & 3) * TC_KCH, row);
         }
@@ -338,8 +343,26 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
   const float** w_src = s_src + wg * WG_ROWS;
   auto wg_bar = [&] { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); };
   const int n_rows = lin ? P.lin_rows : P.g.E;
+  // Chunks this warpgroup has read.  With two consumer warpgroups the ring also carries the other warpgroup's 8 chunks
+  // between two GEMMs of this one; 8 chunks fill each stage an even number of times, so the stage and the parity of a
+  // chunk follow from this count alone.
   uint32_t u = 0;
   float acc[128];
+
+  // Turn-taking of the two consumer warpgroups (named barriers 3 and 4, one per warpgroup).  GEMMs run in ring order,
+  // warpgroup 0's and warpgroup 1's alternating, so each warpgroup's GEMM is preceded by one of the other's.  A warpgroup
+  // enters its GEMM on its own barrier (bar.sync, 256 threads), which the other warpgroup's bar.arrive completes once its
+  // own GEMM has drained.  By then the ring has delivered the two chunks before this GEMM's first two, so each stage is
+  // at most one phase ahead of a parity wait on it.  These waits need no watchdog: the other warpgroup reaches its
+  // bar.arrive through bounded mbarrier waits only.  Warpgroup 1 opens warpgroup 0's first turn; its pass after its last
+  // GEMM is left unmatched when the CTA exits.  (Taking it after the tile loop made ptxas spill three times as much.)
+  auto turn_wait = [&] {
+    if constexpr (NWG == 2) asm volatile("bar.sync %0, 256;" ::"r"(3 + wg) : "memory");
+  };
+  auto turn_pass = [&] {
+    if constexpr (NWG == 2) asm volatile("bar.arrive %0, 256;" ::"r"(4 - wg) : "memory");
+  };
+  if (wg == 1) turn_pass();
 
   // phase timers (TIMED only): thread 0 of the warpgroup adds each phase's cycles straight into P.phase_cycles (fire-
   // and-forget reductions), so the timers keep two 32-bit clock readings in registers (differences of the low clock
@@ -362,8 +385,11 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
   // 8 weight chunks (4 K-chunks x hi, lo) against this warpgroup's A operand (hi, lo at chunk 2 kc, 2 kc + 1).
   // One wgmma group stays in flight across chunk boundaries: chunk i is issued before chunk i - 1's stage is released,
   // so the wait for chunk i + 1's weights overlaps chunk i's tensor work.  The wgmmas still run in issue order on acc.
+  // The time spent waiting for the turn is left out of every phase slot.
   auto gemm = [&](int wait_slot, int mma_slot) {
     uint32_t waited = 0;
+    turn_wait();
+    if constexpr (TIMED) t_mark = (uint32_t)clock();
     acc_fence(acc);
     wgmma_fence();
     int s_prev = 0;
@@ -394,6 +420,7 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
     acc_fence(acc);
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[s_prev]);
+    turn_pass();
     if constexpr (TIMED) {
       const uint32_t now = (uint32_t)clock();
       record(wait_slot, waited);

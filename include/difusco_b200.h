@@ -205,7 +205,8 @@ int dfb_debug_gnn_layer(dfb_ctx* ctx, int layer, float t, float* h, float* e, vo
  * Slots, each summed over every consumer warpgroup of every launch (SM clock cycles):
  *   0 tiles, 1 total cycles of the tile loop, 2 row table + conversion, 3 GEMM1 weight waits, 4 GEMM1 wgmma issue and
  *   drain, 5 gathers + gate + messages, 6 message reduction, 7 LayerNorms + SiLU, 8 GEMM2 weight waits, 9 GEMM2 wgmma
- *   issue and drain, 10 residual update.  Slots 2..10 partition the tile loop, so their sum is at most slot 1. */
+ *   issue and drain, 10 residual update.  Slots 2..10 partition the tile loop except for the waits of a warpgroup for its
+ *   turn on the tensor cores, so their sum is at most slot 1 and the difference is the turn waits. */
 int dfb_debug_phase_cycles(dfb_ctx* ctx, unsigned long long* out);
 
 /* Tuning hook: enabled != 0 routes the product edge-layer launches to a copy of the kernel with phase timers (same

@@ -6,6 +6,8 @@ k = 50, 16 instances, E = 400 000) with the phase timers of k_edge_layer_wg2_tim
 Cycles are SM clock cycles read by thread 0 of each consumer warpgroup and summed over every warpgroup and layer;
 per_tile divides by the tiles each warpgroup processed, so it is the time one warpgroup spends on one tile.  The timed
 kernel is a copy of the product kernel with clock reads added; its outputs are identical, its speed a little lower.
+The phases partition the tile loop except for the waits of a warpgroup for its turn on the tensor cores (the other
+warpgroup's GEMM), which no phase slot holds: turn_wait is the rest of the loop's cycles.
 """
 import argparse
 import json
@@ -78,7 +80,8 @@ def main():
           "cycles_per_tile": total / tiles,
           "per_tile": {k: v / tiles for k, v in phases.items()},
           "share": {k: v / total for k, v in phases.items()},
-          "unaccounted_share": 1.0 - sum(phases.values()) / total,
+          "turn_wait_per_tile": (total - sum(phases.values())) / tiles,
+          "turn_wait_share": 1.0 - sum(phases.values()) / total,
           "gpu": gpu_info()}
   print(json.dumps(line))
 

@@ -16,7 +16,7 @@ AGGREGATION = {"sum": 0, "mean": 1, "max": 2}
 # every symbol include/difusco_b200.h declares (tests check the library exports all of them)
 SYMBOLS = [
     "dfb_abi_version", "dfb_create", "dfb_destroy", "dfb_last_error", "dfb_set_aggregation",
-    "dfb_set_edge_impl", "dfb_load_weights", "dfb_prepare_graph", "dfb_set_points",
+    "dfb_set_edge_impl", "dfb_load_weights", "dfb_prepare_graph", "dfb_prepare_graph_instances", "dfb_set_points",
     "dfb_encoder_forward", "dfb_denoise_step", "dfb_denoise", "dfb_denoise_record", "dfb_denoise_host",
     "dfb_launch_count", "dfb_profile_begin", "dfb_profile_end", "dfb_debug_edge_gemm", "dfb_debug_gnn_layer",
     "dfb_debug_phase_cycles", "dfb_debug_watchdog", "dfb_knn_graph", "dfb_set_graph_capture",
@@ -46,6 +46,7 @@ def lib():
   L.dfb_load_weights.argtypes = [vp, i32, i32, i32, i32, i32, C.POINTER(C.c_char_p), C.POINTER(vp),
                                  C.POINTER(i64)]
   L.dfb_prepare_graph.argtypes = [vp, vp, i64, i64, i32, vp]
+  L.dfb_prepare_graph_instances.argtypes = [vp, vp, i64, i64, i32, C.POINTER(i64), vp]
   L.dfb_set_points.argtypes = [vp, vp, vp]
   L.dfb_encoder_forward.argtypes = [vp, vp, f32, vp, vp]
   L.dfb_denoise_step.argtypes = [vp, i32, vp, f32, C.POINTER(f32), i32, vp, u64, i32, vp, vp, vp, vp]
@@ -200,6 +201,12 @@ class Context(object):
   # ---- graph ----
   def prepare_graph(self, edge_index_ptr, num_nodes, num_edges, gn_segments=1, stream=0):
     self._ck(lib().dfb_prepare_graph(self._h, edge_index_ptr, num_nodes, num_edges, gn_segments, stream))
+
+  def prepare_graph_instances(self, edge_index_ptr, num_nodes, num_edges, node_ptr, stream=0):
+    """One GroupNorm segment per instance; node_ptr: host int64 array of n_instances + 1 node offsets."""
+    node_ptr = np.ascontiguousarray(node_ptr, dtype=np.int64)
+    self._ck(lib().dfb_prepare_graph_instances(self._h, edge_index_ptr, num_nodes, num_edges, node_ptr.size - 1,
+                                               node_ptr.ctypes.data_as(C.POINTER(C.c_int64)), stream))
 
   def set_points(self, points_ptr, stream=0):
     self._ck(lib().dfb_set_points(self._h, points_ptr, stream))

@@ -51,8 +51,9 @@ struct dfb_ctx {
   // ---- graph ----
   bool graph_ready = false, points_ready = false;
   GraphDev g{};
-  int gn_segments = 1;
-  DevBuf d_row, d_col, d_perm, d_rowptr, d_grp_first, d_grp_pair, d_ei_stage;
+  GnSegments gseg{};      // head GroupNorm segments (kernels_small.cuh)
+  int gn_blocks = 0;      // k_gn_partial blocks over all segments
+  DevBuf d_row, d_col, d_perm, d_rowptr, d_grp_first, d_grp_pair, d_ei_stage, d_seg_start, d_seg_blk_first, d_gn_blk;
   // ---- workspace ----
   DevBuf e, h, h0, uvab, uvab0, partials, feat, tvec, tvals, gn_part, gn_stats, d_points, d_xt, d_u;
   DevBuf opt_points, opt_tours, opt_pos, opt_dnext, opt_cand, opt_tiles, opt_state, opt_best;   // 2-opt (row f3)
@@ -459,19 +460,30 @@ extern "C" int dfb_set_aggregation(dfb_ctx* ctx, int mode) {
 // ================================================================================================
 // graph
 // ================================================================================================
-extern "C" int dfb_prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_t V64, int64_t E64,
-                                 int gn_segments, void* stream_) {
+// dfb_prepare_graph (node_ptr null: gn_segments equal row blocks) and dfb_prepare_graph_instances (node_ptr[n_inst + 1]:
+// one segment per instance).  Every argument is checked before any context state changes, so a rejected call leaves
+// the previously prepared graph in use.
+static int prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_t V64, int64_t E64, int gn_segments,
+                         int n_inst, const int64_t* node_ptr, cudaStream_t st) {
   if (!ctx) return DFB_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream_;
   CK(ctx, cudaSetDevice(ctx->device));
   if (!ctx->weights_loaded) FAIL(ctx, DFB_E_INVALID, "dfb_load_weights must be called first");
   if (V64 <= 0 || E64 <= 0 || V64 > 0x7fffffff / 4 || E64 > 0x7ffffff0)
     FAIL(ctx, DFB_E_INVALID, "bad graph size V=%lld E=%lld", (long long)V64, (long long)E64);
   const int V = (int)V64, E = (int)E64;
-  if (gn_segments < 1) FAIL(ctx, DFB_E_INVALID, "gn_segments must be >= 1");
-  {
-    int R = ctx->node_only ? V : E;
+  const int R = ctx->node_only ? V : E;   // rows of the head
+  if (!node_ptr) {
+    if (gn_segments < 1) FAIL(ctx, DFB_E_INVALID, "gn_segments must be >= 1");
     if (R % gn_segments) FAIL(ctx, DFB_E_INVALID, "gn_segments %d does not divide %d rows", gn_segments, R);
+  } else {
+    if (n_inst < 1) FAIL(ctx, DFB_E_INVALID, "n_instances %d < 1", n_inst);
+    if (node_ptr[0] != 0 || node_ptr[n_inst] != V64)
+      FAIL(ctx, DFB_E_INVALID, "node_ptr must run from 0 to num_nodes %lld (got %lld .. %lld)", (long long)V64,
+           (long long)node_ptr[0], (long long)node_ptr[n_inst]);
+    for (int i = 0; i < n_inst; ++i)
+      if (node_ptr[i + 1] <= node_ptr[i])
+        FAIL(ctx, DFB_E_INVALID, "node_ptr must be strictly increasing (instance %d: %lld after %lld)", i,
+             (long long)node_ptr[i + 1], (long long)node_ptr[i]);
   }
   std::vector<int64_t> stage;
   const int64_t* ei = edge_index;
@@ -483,16 +495,45 @@ extern "C" int dfb_prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_
   }
   const int64_t* row64 = ei;
   const int64_t* col64 = ei + E;
+  std::vector<int> inst;   // instance of each node
+  if (node_ptr) {
+    inst.resize(V);
+    for (int i = 0; i < n_inst; ++i)
+      for (int64_t v = node_ptr[i]; v < node_ptr[i + 1]; ++v) inst[v] = i;
+  }
   std::vector<int> rowptr((size_t)V + 1, 0);
   bool sorted = true;
   for (int s = 0; s < E; ++s) {
     int64_t r = row64[s], c = col64[s];
     if (r < 0 || r >= V || c < 0 || c >= V)
       FAIL(ctx, DFB_E_INVALID, "edge %d = (%lld,%lld) out of range for %d nodes", s, (long long)r, (long long)c, V);
+    if (node_ptr && inst[r] != inst[c])
+      FAIL(ctx, DFB_E_INVALID, "edge %d = (%lld,%lld) joins instances %d and %d", s, (long long)r, (long long)c,
+           inst[r], inst[c]);
     rowptr[(size_t)r + 1]++;
     if (s && r < row64[s - 1]) sorted = false;
   }
   for (int i = 0; i < V; ++i) rowptr[i + 1] += rowptr[i];
+  // segment table: the first head row of each segment (TSP: rows of the row-sorted edge order, so instance i starts
+  // at rowptr[node_ptr[i]]; MIS: node rows), then the k_gn_partial blocks of each segment
+  const int S = node_ptr ? n_inst : gn_segments;
+  std::vector<int> seg_start((size_t)S + 1), blk_first((size_t)S + 1);
+  for (int i = 0; i <= S; ++i) {
+    if (!node_ptr) seg_start[i] = (int)((int64_t)R / S * i);
+    else seg_start[i] = ctx->node_only ? (int)node_ptr[i] : rowptr[node_ptr[i]];
+  }
+  for (int i = 0; i < S; ++i)
+    if (seg_start[i + 1] == seg_start[i])   // only a TSP instance can have no head rows
+      FAIL(ctx, DFB_E_INVALID, "instance %d (nodes %lld..%lld) has no edges: its GroupNorm would be over zero rows", i,
+           (long long)node_ptr[i], (long long)node_ptr[i + 1] - 1);
+  std::vector<int2> gn_blk;
+  for (int i = 0; i < S; ++i) {
+    blk_first[i] = (int)gn_blk.size();
+    for (int r0 = seg_start[i]; r0 < seg_start[i + 1]; r0 += GN_ROWS_PER_BLOCK) gn_blk.push_back(make_int2(i, r0));
+  }
+  blk_first[S] = (int)gn_blk.size();
+  const int nb = (int)gn_blk.size();
+
   std::vector<int> row(E), col(E), perm;
   if (sorted) {
     for (int s = 0; s < E; ++s) {
@@ -534,6 +575,12 @@ extern "C" int dfb_prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_
     ENS(ctx, ctx->d_perm, (size_t)E * 4);
     CK(ctx, cudaMemcpyAsync(ctx->d_perm.p, perm.data(), (size_t)E * 4, cudaMemcpyHostToDevice, st));
   }
+  ENS(ctx, ctx->d_seg_start, ((size_t)S + 1) * 4);
+  ENS(ctx, ctx->d_seg_blk_first, ((size_t)S + 1) * 4);
+  ENS(ctx, ctx->d_gn_blk, (size_t)nb * sizeof(int2));
+  CK(ctx, cudaMemcpyAsync(ctx->d_seg_start.p, seg_start.data(), ((size_t)S + 1) * 4, cudaMemcpyHostToDevice, st));
+  CK(ctx, cudaMemcpyAsync(ctx->d_seg_blk_first.p, blk_first.data(), ((size_t)S + 1) * 4, cudaMemcpyHostToDevice, st));
+  CK(ctx, cudaMemcpyAsync(ctx->d_gn_blk.p, gn_blk.data(), (size_t)nb * sizeof(int2), cudaMemcpyHostToDevice, st));
   CK(ctx, cudaStreamSynchronize(st));   // host vectors go out of scope
   GraphDev& g = ctx->g;
   g.V = V; g.E = E;
@@ -542,7 +589,11 @@ extern "C" int dfb_prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_
   g.rowptr = (const int*)ctx->d_rowptr.p;
   g.n_groups = nG; g.grp_first = (const int*)ctx->d_grp_first.p; g.grp_pair = (const int*)ctx->d_grp_pair.p;
   g.n_pairs = np;
-  ctx->gn_segments = gn_segments;
+  ctx->gseg.n_segs = S;
+  ctx->gseg.start = (const int*)ctx->d_seg_start.p;
+  ctx->gseg.blk_first = (const int*)ctx->d_seg_blk_first.p;
+  ctx->gseg.blk = (const int2*)ctx->d_gn_blk.p;
+  ctx->gn_blocks = nb;
 
   // workspace
   ENS(ctx, ctx->e, (size_t)E * H * sizeof(float));
@@ -553,18 +604,24 @@ extern "C" int dfb_prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_
   ENS(ctx, ctx->partials, (size_t)np * H * sizeof(float));
   const size_t feat_rows = 65536;
   ENS(ctx, ctx->feat, feat_rows * H * sizeof(float));
-  {
-    int R = ctx->node_only ? V : E;
-    int rps = R / gn_segments;
-    int bps = (rps + GN_ROWS_PER_BLOCK - 1) / GN_ROWS_PER_BLOCK;
-    ENS(ctx, ctx->gn_part, std::max((size_t)gn_segments * bps, (size_t)1024) * 32 * 2 * sizeof(double));
-    ENS(ctx, ctx->gn_stats, (size_t)gn_segments * 32 * 2 * sizeof(float));
-  }
+  ENS(ctx, ctx->gn_part, std::max((size_t)nb, (size_t)1024) * 32 * 2 * sizeof(double));
+  ENS(ctx, ctx->gn_stats, (size_t)S * 32 * 2 * sizeof(float));
   ENS(ctx, ctx->d_xt, (size_t)std::max(V, E) * sizeof(float));
   ctx->graph_ready = true;
   ctx->buf_gen++;
   ctx->points_ready = false;
   return DFB_OK;
+}
+
+extern "C" int dfb_prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_t num_nodes, int64_t num_edges,
+                                 int gn_segments, void* stream) {
+  return prepare_graph(ctx, edge_index, num_nodes, num_edges, gn_segments, 0, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int dfb_prepare_graph_instances(dfb_ctx* ctx, const int64_t* edge_index, int64_t num_nodes,
+                                           int64_t num_edges, int n_instances, const int64_t* node_ptr, void* stream) {
+  if (ctx && !node_ptr) FAIL(ctx, DFB_E_INVALID, "node_ptr is required");
+  return prepare_graph(ctx, edge_index, num_nodes, num_edges, 0, n_instances, node_ptr, (cudaStream_t)stream);
 }
 
 // What dfb_set_edge_impl selects for the linears and edge layers: the fp32 FFMA kernels (validation), or the
@@ -744,15 +801,13 @@ static int run_forward(dfb_ctx* ctx, const float* xt, const float* tvec, bool bi
   // head
   const float* Z = ctx->node_only ? h : e;
   const int R = ctx->node_only ? V : E;
-  const int rps = R / ctx->gn_segments;
-  const int bps = (rps + GN_ROWS_PER_BLOCK - 1) / GN_ROWS_PER_BLOCK;
-  k_gn_partial<<<dim3(bps, ctx->gn_segments), 256, 0, st>>>(Z, rps, (double*)ctx->gn_part.p);
+  k_gn_partial<<<ctx->gn_blocks, 256, 0, st>>>(Z, ctx->gseg, (double*)ctx->gn_part.p);
   CKL(ctx);
-  k_gn_final<<<dim3(ctx->gn_segments, 32), 256, 0, st>>>((const double*)ctx->gn_part.p, Z, bps, rps,
-                                                      (float*)ctx->gn_stats.p);
+  k_gn_final<<<dim3(ctx->gseg.n_segs, 32), 256, 0, st>>>((const double*)ctx->gn_part.p, Z, ctx->gseg,
+                                                         (float*)ctx->gn_stats.p);
   CKL(ctx);
-  k_head<<<(R + 255) / 256, 256, 0, st>>>(Z, R, rps, (const float*)ctx->gn_stats.p, ctx->node_only ? nullptr : g.perm,
-                                      ctx->hp, pa);
+  k_head<<<(R + 255) / 256, 256, 0, st>>>(Z, R, ctx->gseg, (const float*)ctx->gn_stats.p,
+                                      ctx->node_only ? nullptr : g.perm, ctx->hp, pa);
   CKL(ctx);
   return DFB_OK;
 }

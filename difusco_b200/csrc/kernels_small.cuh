@@ -195,23 +195,32 @@ __global__ void __launch_bounds__(256) k_node_update(float* __restrict__ h, cons
 // ---------------------------------------------------------------------------------------------
 // Head GroupNorm32(32, 256) statistics over ALL rows of a segment (gnn_encoder.py:400-401: the
 // batch dim is 1, so every edge of the call shares the statistics; nn.py:17-19).
+// A segment is a run of consecutive head rows normalised on its own: one per call, one per dense sample, or one per
+// instance of a ragged batch (dfb_prepare_graph_instances).  GnSegments holds the table dfb_prepare_graph builds.
 // fp32 runs of <= 32 rows, combined in fp64 partials: 3.2 M values per group would lose the 1e-4 contract in fp32
 // E[x^2]-E[x]^2 form (the reference's own CPU channels-last kernel does lose it when |mean|>>std).  The runs sum
 // x - pivot, with one pivot per (segment, group): the group's first channel in the segment's first row.  Without it
 // the fp32 runs of x^2 round at |mean|^2 * 2^-24, which is the whole variance once |mean| / std reaches ~1000.
 // ---------------------------------------------------------------------------------------------
 constexpr int GN_ROWS_PER_BLOCK = 256;
-__device__ __forceinline__ float gn_pivot(const float* Z, int seg, int rows_per_seg, int group) {
-  return Z[(size_t)seg * rows_per_seg * H + group * 8];
+struct GnSegments {
+  int n_segs;
+  const int* start;       // [n_segs + 1] first head row of each segment; start[n_segs] = rows of the call
+  const int* blk_first;   // [n_segs + 1] first k_gn_partial block of each segment; blk_first[n_segs] = block count
+  const int2* blk;        // [block count] {segment, first row}: GN_ROWS_PER_BLOCK rows counted from the segment's start
+};
+__device__ __forceinline__ float gn_pivot(const float* Z, int seg_row0, int group) {
+  return Z[(size_t)seg_row0 * H + group * 8];
 }
-__global__ void __launch_bounds__(256) k_gn_partial(const float* __restrict__ Z, int rows_per_seg,
+__global__ void __launch_bounds__(256) k_gn_partial(const float* __restrict__ Z, GnSegments sg,
                                                     double* __restrict__ part) {
-  // grid (blocks_per_seg, segs).  thread = channel; fp32 run of <= 32 rows, then fp64.
-  int seg = blockIdx.y, c = threadIdx.x;
-  int r0 = blockIdx.x * GN_ROWS_PER_BLOCK;
-  int r1 = min(r0 + GN_ROWS_PER_BLOCK, rows_per_seg);
-  const float* base = Z + ((size_t)seg * rows_per_seg) * H + c;
-  const float piv = gn_pivot(Z, seg, rows_per_seg, c >> 3);
+  // one block per entry of sg.blk.  thread = channel; fp32 run of <= 32 rows, then fp64.
+  const int c = threadIdx.x;
+  const int2 bk = sg.blk[blockIdx.x];
+  const int r0 = bk.y;
+  const int r1 = min(r0 + GN_ROWS_PER_BLOCK, sg.start[bk.x + 1]);
+  const float* base = Z + c;
+  const float piv = gn_pivot(Z, sg.start[bk.x], c >> 3);
   double S = 0.0, Q = 0.0;
   for (int r = r0; r < r1; r += 32) {
     float s = 0.f, q = 0.f;
@@ -231,21 +240,21 @@ __global__ void __launch_bounds__(256) k_gn_partial(const float* __restrict__ Z,
     Q += __shfl_xor_sync(0xffffffffu, Q, o);
   }
   if ((c & 7) == 0) {
-    size_t o = (((size_t)seg * gridDim.x + blockIdx.x) * 32 + (c >> 3)) * 2;
+    size_t o = ((size_t)blockIdx.x * 32 + (c >> 3)) * 2;
     part[o] = S;
     part[o + 1] = Q;
   }
 }
 __global__ void __launch_bounds__(256) k_gn_final(const double* __restrict__ part, const float* __restrict__ Z,
-                                                  int blocks_per_seg, int rows_per_seg,
-                                                  float* __restrict__ stats /* [segs][32][2] mean, rstd */) {
-  // grid (segs, 32 groups); 256 threads stride over the per-block partials, then a fixed-shape fp64 tree
+                                                  GnSegments sg, float* __restrict__ stats /* [segs][32][2] mean, rstd */) {
+  // grid (segs, 32 groups); 256 threads stride over the segment's block partials, then a fixed-shape fp64 tree
   // (warp shuffles + 8 warp results in shared memory): deterministic
   __shared__ double sh[8][2];
   const int seg = blockIdx.x, gidx = blockIdx.y, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int b0 = sg.blk_first[seg], nb = sg.blk_first[seg + 1] - b0;
   double S = 0.0, Q = 0.0;
-  for (int b = threadIdx.x; b < blocks_per_seg; b += 256) {
-    size_t o = (((size_t)seg * blocks_per_seg + b) * 32 + gidx) * 2;
+  for (int b = threadIdx.x; b < nb; b += 256) {
+    size_t o = (((size_t)b0 + b) * 32 + gidx) * 2;
     S += part[o];
     Q += part[o + 1];
   }
@@ -256,12 +265,13 @@ __global__ void __launch_bounds__(256) k_gn_final(const double* __restrict__ par
   if (threadIdx.x == 0) {
     S = 0.0; Q = 0.0;
     for (int i = 0; i < 8; ++i) { S += sh[i][0]; Q += sh[i][1]; }
-    double n = (double)rows_per_seg * 8.0;
+    const int s0 = sg.start[seg];
+    double n = (double)(sg.start[seg + 1] - s0) * 8.0;
     double dm = S / n;                       // mean - pivot
     double var = Q / n - dm * dm;
     if (var < 0.0) var = 0.0;
-    stats[(seg * 32 + gidx) * 2] = (float)((double)gn_pivot(Z, seg, rows_per_seg, gidx) + dm);
-    stats[(seg * 32 + gidx) * 2 + 1] = (float)(1.0 / sqrt(var + (double)LN_EPS));
+    stats[((size_t)seg * 32 + gidx) * 2] = (float)((double)gn_pivot(Z, s0, gidx) + dm);
+    stats[((size_t)seg * 32 + gidx) * 2 + 1] = (float)(1.0 / sqrt(var + (double)LN_EPS));
   }
 }
 
@@ -357,7 +367,7 @@ __device__ __forceinline__ void head_posterior(const HeadParams& hp, const Poste
 // A warp takes 32 consecutive rows: lane == GroupNorm group (8 channels) for the per-row partial dot products,
 // then a butterfly transpose-reduce (31 shuffles per output channel for all 32 rows) leaves row j's logits in
 // lane j, so the softmax / posterior / Philox epilogue runs on all 32 lanes in parallel.
-__global__ void __launch_bounds__(256, 2) k_head(const float* __restrict__ Z, int R, int rows_per_seg,
+__global__ void __launch_bounds__(256, 2) k_head(const float* __restrict__ Z, int R, GnSegments sg,
                                               const float* __restrict__ stats,
                                               const int* __restrict__ perm, HeadParams hp,
                                               PosteriorArgs pa) {
@@ -374,17 +384,25 @@ __global__ void __launch_bounds__(256, 2) k_head(const float* __restrict__ Z, in
     w0[j] = hp.W[c];
     w1[j] = (hp.out_channels == 2) ? hp.W[H + c] : 0.0f;
   }
+  // segment of the warp's first row: binary search over the segment starts (no load for one segment).  Every segment
+  // has a row, so each following row is in the same segment or starts the next one.  All of it is warp-uniform.
+  int seg = 0;
+  for (int hi = sg.n_segs; hi - seg > 1;) {
+    const int mid = (seg + hi) >> 1;
+    if (sg.start[mid] <= r0) seg = mid; else hi = mid;
+  }
+  int seg_end = sg.start[seg + 1];
+  float mean = stats[((size_t)seg * 32 + lane) * 2];
+  float rstd = stats[((size_t)seg * 32 + lane) * 2 + 1];
   float a0[32], a1[32];
-  int seg_prev = -1;
-  float mean = 0.f, rstd = 0.f;
 #pragma unroll
   for (int i = 0; i < 32; ++i) {
     const int r = min(r0 + i, R - 1);
-    const int seg = r / rows_per_seg;
-    if (seg != seg_prev) {   // warp-uniform
-      mean = stats[(seg * 32 + lane) * 2];
-      rstd = stats[(seg * 32 + lane) * 2 + 1];
-      seg_prev = seg;
+    if (r >= seg_end) {   // warp-uniform
+      ++seg;
+      seg_end = sg.start[seg + 1];
+      mean = stats[((size_t)seg * 32 + lane) * 2];
+      rstd = stats[((size_t)seg * 32 + lane) * 2 + 1];
     }
     const float4* zp = reinterpret_cast<const float4*>(Z + (size_t)r * H) + lane * 2;
     const float4 x0 = __ldcs(zp), x1 = __ldcs(zp + 1);

@@ -14,6 +14,10 @@ Interface notes (reference behaviour kept):
     evaluated as the row-major complete graph incl. self pairs (gnn_encoder.py:365 makes the
     graph all-ones), GroupNorm per sample.
   * dense + node_feature_only raises NotImplementedError (:457), as in the reference.
+  * sparse TSP and MIS take a keyword-only node_ptr (PyG's Batch.ptr: instance i owns nodes
+    [node_ptr[i], node_ptr[i+1])): one block-diagonal call over a ragged batch whose head GroupNorm
+    runs per instance, so every instance gets the result it would get alone (the reference's test
+    loader runs batch size 1).  Without it the GroupNorm statistics span every row of the call.
 Only inference is in scope: per-edge timestep vectors (training, pl_tsp_model.py:66-68) raise
 NotImplementedError; autograd is not supported - outputs carry no grad_fn, and a call with grad mode
 enabled on parameters that require grad warns once.
@@ -38,6 +42,22 @@ def reference_frequency_tables(hidden_dim):
   dimt_scalar = 10000 ** (2 * torch.div(i, 2, rounding_mode="trunc") / hidden_dim)
   return {"__const.time_freqs": freqs.numpy(), "__const.dimt_pos": dimt_pos.numpy(),
           "__const.dimt_scalar": dimt_scalar.numpy()}
+
+
+def node_ptr_array(node_ptr):
+  """node_ptr, a 1-D integer tensor or sequence of n_instances + 1 node offsets (PyG's Batch.ptr) -> host int64
+  numpy array.  Checks its shape and dtype; dfb_prepare_graph_instances checks the offsets against the graph."""
+  if isinstance(node_ptr, torch.Tensor):
+    if node_ptr.dtype not in (torch.int8, torch.int16, torch.int32, torch.int64, torch.uint8):
+      raise ValueError(f"node_ptr must hold integers, got {node_ptr.dtype}")
+    a = node_ptr.detach().cpu().numpy()
+  else:
+    a = np.asarray(node_ptr)
+    if a.dtype.kind not in "iu":
+      raise ValueError(f"node_ptr must hold integers, got {a.dtype}")
+  if a.ndim != 1 or a.shape[0] < 2:
+    raise ValueError(f"node_ptr must be 1-D with n_instances + 1 >= 2 entries, got shape {tuple(a.shape)}")
+  return np.ascontiguousarray(a, dtype=np.int64)
 
 
 class GNNLayer(nn.Module):
@@ -132,15 +152,23 @@ class GNNEncoder(nn.Module):
   def _stream():
     return torch.cuda.current_stream().cuda_stream
 
-  def set_graph(self, edge_index, num_nodes, gn_segments=1):
-    """Prepare (and cache) the graph of subsequent calls.  edge_index (2,E) int64, any device."""
+  def set_graph(self, edge_index, num_nodes, gn_segments=1, node_ptr=None):
+    """Prepare (and cache) the graph of subsequent calls.  edge_index (2,E) int64, any device.  The head GroupNorm
+    runs over gn_segments equal row blocks, or, with node_ptr (n_instances + 1 node offsets), once per instance."""
+    ptr = None if node_ptr is None else node_ptr_array(node_ptr)
+    if ptr is not None and int(gn_segments) != 1:
+      raise ValueError("give node_ptr or gn_segments, not both")
     ctx = self.engine()
     ei = edge_index.long().contiguous()
-    key = (ei.data_ptr(), tuple(ei.shape), ei._version, int(num_nodes), int(gn_segments), str(ei.device))
+    key = (ei.data_ptr(), tuple(ei.shape), ei._version, int(num_nodes), int(gn_segments), str(ei.device),
+           None if ptr is None else ptr.tobytes())
     if key != self._graph_key:
       if ei.dim() != 2 or ei.shape[0] != 2:
         raise ValueError("edge_index must have shape (2, E)")
-      ctx.prepare_graph(ei.data_ptr(), int(num_nodes), int(ei.shape[1]), int(gn_segments), self._stream())
+      if ptr is None:
+        ctx.prepare_graph(ei.data_ptr(), int(num_nodes), int(ei.shape[1]), int(gn_segments), self._stream())
+      else:
+        ctx.prepare_graph_instances(ei.data_ptr(), int(num_nodes), int(ei.shape[1]), ptr, self._stream())
       self._graph_key = key
       self._graph_hold = ei
       self._points_key = None
@@ -175,18 +203,18 @@ class GNNEncoder(nn.Module):
   # ------------------------------------------------------------------------------------------
   # forward variants (gnn_encoder.py:350-462)
   # ------------------------------------------------------------------------------------------
-  def sparse_forward(self, x, graph, timesteps, edge_index):
+  def sparse_forward(self, x, graph, timesteps, edge_index, node_ptr=None):
     V, E = x.shape[0], edge_index.shape[1]
-    ctx = self.set_graph(edge_index, V, 1)
+    ctx = self.set_graph(edge_index, V, 1, node_ptr)
     self.set_points(x.to(self._device()))
     xt = graph.reshape(-1).float().contiguous().to(self._device())
     out = torch.empty((E, self.out_channels), device=self._device(), dtype=torch.float32)
     ctx.encoder_forward(xt.data_ptr(), self._single_t(timesteps), out.data_ptr(), self._stream())
     return out
 
-  def sparse_forward_node_feature_only(self, x, timesteps, edge_index):
+  def sparse_forward_node_feature_only(self, x, timesteps, edge_index, node_ptr=None):
     V = x.shape[0]
-    ctx = self.set_graph(edge_index, V, 1)
+    ctx = self.set_graph(edge_index, V, 1, node_ptr)
     xt = x.reshape(-1).float().contiguous().to(self._device())
     out = torch.empty((V, self.out_channels), device=self._device(), dtype=torch.float32)
     ctx.encoder_forward(xt.data_ptr(), self._single_t(timesteps), out.data_ptr(), self._stream())
@@ -211,7 +239,11 @@ class GNNEncoder(nn.Module):
         out[b:b + 1] = self.dense_forward(x[b:b + 1], graph[b:b + 1], t[b:b + 1])
     return out
 
-  def forward(self, x, timesteps, graph=None, edge_index=None):
+  def forward(self, x, timesteps, graph=None, edge_index=None, *, node_ptr=None):
+    """node_ptr (sparse TSP and MIS only): node offsets of the instances of a block-diagonal batch, each of which
+    then gets its own head GroupNorm.  The dense forward already normalises each sample on its own."""
+    if node_ptr is not None and not self.sparse:
+      raise ValueError("node_ptr is for sparse graphs: the dense forward already normalises each sample on its own")
     if torch.is_grad_enabled() and not GNNEncoder._warned_no_grad and any(p.requires_grad for p in self.parameters()):
       # inference engine: never builds an autograd graph; make misuse visible (once)
       import warnings
@@ -220,8 +252,8 @@ class GNNEncoder(nn.Module):
       GNNEncoder._warned_no_grad = True
     if self.node_feature_only:
       if self.sparse:
-        return self.sparse_forward_node_feature_only(x, timesteps, edge_index)
+        return self.sparse_forward_node_feature_only(x, timesteps, edge_index, node_ptr)
       raise NotImplementedError
     if self.sparse:
-      return self.sparse_forward(x, graph, timesteps, edge_index)
+      return self.sparse_forward(x, graph, timesteps, edge_index, node_ptr)
     return self.dense_forward(x, graph, timesteps, edge_index)

@@ -32,13 +32,15 @@ class MISModel(COMetaModel):
   def gaussian_denoise_step(self, xt, t, device, edge_index=None, target_t=None):
     return self._denoise_step(xt, t, device, edge_index, target_t)
 
-  def denoise_labels(self, edge_index, xt, steps=None, seed=None, record_steps=None):
+  def denoise_labels(self, edge_index, xt, steps=None, seed=None, record_steps=None, node_ptr=None):
     """xt0 (V,) -> raw final node labels on device, the whole loop fused.  record_steps (step indices or "all"):
-    returns (labels, trace) instead, trace as COMetaModel._fused_loop: "xt" / "p" (n_rec, V), "out" (n_rec, V, out)."""
+    returns (labels, trace) instead, trace as COMetaModel._fused_loop: "xt" / "p" (n_rec, V), "out" (n_rec, V, out).
+    node_ptr: node offsets of the graphs of a block-diagonal batch (PyG's Batch.ptr); each graph then gets its own
+    head GroupNorm, as if it were denoised alone."""
     steps = steps or self.args.inference_diffusion_steps
     with torch.no_grad():
       dev = self.model._device()
-      self.model.set_graph(edge_index.long().to(dev), xt.shape[0], 1)
+      self.model.set_graph(edge_index.long().to(dev), xt.shape[0], 1, node_ptr)
       x = xt.reshape(-1).float().contiguous().to(dev).clone()
       return self._fused_loop(x, steps, seed, record_steps)
 

@@ -36,13 +36,15 @@ class TSPModel(COMetaModel):
     return self.model(x, t, adj, edge_index)
 
   # ------------------------------------------------------------------------------------
-  def _prepare(self, points, edge_index, device):
+  def _prepare(self, points, edge_index, device, node_ptr=None):
     """Make self.model's engine hold this call's graph + coordinates; returns dense batch B or 0."""
     if self.sparse:
       V = points.shape[0]
-      self.model.set_graph(edge_index.long().to(device), V, 1)
+      self.model.set_graph(edge_index.long().to(device), V, 1, node_ptr)
       self.model.set_points(points.float().to(device))
       return 0
+    if node_ptr is not None:
+      raise ValueError("node_ptr is for sparse graphs: the dense path already normalises each sample on its own")
     B, V, _ = points.shape
     self.model.set_graph(self.model._complete_graph(B, V, device), B * V, B)
     self.model.set_points(points.reshape(B * V, 2).float().to(device))
@@ -62,8 +64,12 @@ class TSPModel(COMetaModel):
     return self._denoise_step(points, xt, t, device, edge_index, target_t)
 
   # ------------------------------------------------------------------------------------
-  def denoise_heatmap(self, points, edge_index, xt, steps=None, seed=None, record_steps=None):
+  def denoise_heatmap(self, points, edge_index, xt, steps=None, seed=None, record_steps=None, node_ptr=None):
     """xt0 -> raw final xt on device, the whole loop fused (no host sync inside).
+
+    node_ptr (sparse only): node offsets of the instances of a block-diagonal batch (PyG's Batch.ptr); each instance
+    then gets its own head GroupNorm, as if it were denoised alone.  The sampling draws still depend on an edge's
+    position in the call.
 
     record_steps (step indices or "all"): returns (heatmap, trace) instead, trace as COMetaModel._fused_loop with
     each tensor shaped like xt after its leading step dimension: (n_rec, E) sparse, (n_rec, B, V, V) dense; "out"
@@ -71,7 +77,7 @@ class TSPModel(COMetaModel):
     steps = steps or self.args.inference_diffusion_steps
     with torch.no_grad():
       dev = self.model._device()
-      self._prepare(points.to(dev), edge_index.to(dev) if edge_index is not None else None, dev)
+      self._prepare(points.to(dev), edge_index.to(dev) if edge_index is not None else None, dev, node_ptr)
       x = xt.reshape(-1).float().contiguous().to(dev).clone()
       if record_steps is None:
         self._fused_loop(x, steps, seed)

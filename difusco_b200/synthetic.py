@@ -151,6 +151,12 @@ def mis_batch(n_lo, n_hi, p, batch, seed=0):
   return np.concatenate(eis, 1), sizes
 
 
+def node_ptr(sizes):
+  """Node offsets (PyG's Batch.ptr) of graphs with `sizes` nodes concatenated block-diagonally: (len(sizes) + 1,)
+  int64, node_ptr[i] the first node of graph i."""
+  return np.concatenate([[0], np.cumsum(np.asarray(sizes, np.int64))]).astype(np.int64)
+
+
 # --------------------------------------------------------------------------------------------
 # noise
 # --------------------------------------------------------------------------------------------

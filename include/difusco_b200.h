@@ -77,6 +77,18 @@ int dfb_load_weights(dfb_ctx* ctx, int n_layers, int hidden_dim, int out_channel
 int dfb_prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_t num_nodes, int64_t num_edges,
                       int gn_segments, void* stream);
 
+/* dfb_prepare_graph for a ragged batch of independent graphs in one block-diagonal call, each with its own head
+ * GroupNorm: the reference's answer for every instance as if it were evaluated alone (its test loader's batch size 1,
+ * pl_meta_model.py:194-198), at the throughput of one call.  node_ptr is a HOST array of n_instances + 1 elements in
+ * PyG's Batch.ptr convention: instance i owns nodes [node_ptr[i], node_ptr[i+1]), and its GroupNorm runs over its
+ * edges (TSP) or its nodes (MIS).  edge_index as for dfb_prepare_graph (need not be sorted).  Sampling is not per
+ * instance: the Philox draws stay keyed by the element's index in the call.
+ * DFB_E_INVALID, with the previously prepared graph left in use, when n_instances < 1, node_ptr[0] != 0,
+ * node_ptr[n_instances] != num_nodes, node_ptr is not strictly increasing, an edge joins two instances, or a TSP
+ * instance has no edges. */
+int dfb_prepare_graph_instances(dfb_ctx* ctx, const int64_t* edge_index, int64_t num_nodes, int64_t num_edges,
+                                int n_instances, const int64_t* node_ptr, void* stream);
+
 /* TSP only: node coordinates (V,2) fp32, HOST or DEVICE.  Computes the step-invariant
  * h0 = node_embed(pos_embed(x)) (gnn_encoder.py:394, :211-227) and layer 0's node linears. */
 int dfb_set_points(dfb_ctx* ctx, const float* points, void* stream);

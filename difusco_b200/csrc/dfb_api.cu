@@ -55,20 +55,20 @@ struct dfb_ctx {
   int gn_blocks = 0;      // k_gn_partial blocks over all segments
   DevBuf d_row, d_col, d_perm, d_rowptr, d_grp_first, d_grp_pair, d_ei_stage, d_seg_start, d_seg_blk_first, d_gn_blk;
   // ---- workspace ----
-  DevBuf e, h, h0, uvab, uvab0, partials, feat, tvec, tvals, gn_part, gn_stats, d_points, d_xt, d_u;
+  DevBuf e, h, h0, uvab, uvab0, partials, feat, tvec, gn_part, gn_stats, d_points, d_xt, d_u;
   DevBuf opt_points, opt_tours, opt_pos, opt_dnext, opt_cand, opt_tiles, opt_state, opt_best;   // 2-opt (row f3)
-  int tvec_steps_cap = 0;
   // ---- step staging (pinned) + captured loop ----
   // dfb_denoise_step / dfb_denoise never allocate, never synchronise the host with the stream and never touch the
-  // heap after the first call of a shape: timesteps and posterior constants go through two pinned staging slots
-  // (guarded by an event each), the per-step table lives in device memory, and the whole loop is replayed as ONE
+  // heap after the first call of a shape: timesteps and per-step parameters go through two pinned staging slots
+  // (guarded by an event each) into the device tables tvals / d_steps, and the whole loop is replayed as ONE
   // CUDA graph that is re-captured only when the shape / buffers / implementation change.
   static constexpr int STAGE_SLOTS = 2, MAX_STEPS = 4096;
   float* h_tvals[STAGE_SLOTS] = {nullptr, nullptr};
   StepParams* h_steps[STAGE_SLOTS] = {nullptr, nullptr};
   cudaEvent_t stage_ev[STAGE_SLOTS] = {nullptr, nullptr};
   int stage_next = 0;
-  DevBuf d_steps;
+  float* tvals = nullptr;          // [MAX_STEPS] device twins of the slots
+  StepParams* d_steps = nullptr;   // [MAX_STEPS]
   uint64_t buf_gen = 0;          // bumped whenever a device buffer is (re)allocated or the graph / weights change
   bool capture_enabled = true;
   bool capture_broken = false;
@@ -106,6 +106,8 @@ struct dfb_ctx {
       if (h_steps[i]) cudaFreeHost(h_steps[i]);
       if (stage_ev[i]) cudaEventDestroy(stage_ev[i]);
     }
+    if (tvals) cudaFree(tvals);
+    if (d_steps) cudaFree(d_steps);
   }
 };
 
@@ -223,6 +225,12 @@ extern "C" int dfb_create(dfb_ctx** out, int device) {
       delete ctx;
       return DFB_E_CUDA;
     }
+  }
+  if ((e = cudaMalloc((void**)&ctx->tvals, dfb_ctx::MAX_STEPS * sizeof(float))) != cudaSuccess ||
+      (e = cudaMalloc((void**)&ctx->d_steps, dfb_ctx::MAX_STEPS * sizeof(StepParams))) != cudaSuccess) {
+    g_create_error = std::string("step tables: ") + cudaGetErrorString(e);
+    delete ctx;
+    return DFB_E_NOMEM;
   }
   if ((e = cudaStreamCreateWithFlags(&ctx->loop_stream, cudaStreamNonBlocking)) != cudaSuccess ||
       (e = cudaEventCreateWithFlags(&ctx->loop_in, cudaEventDisableTiming)) != cudaSuccess ||
@@ -436,9 +444,8 @@ extern "C" int dfb_load_weights(dfb_ctx* ctx, int n_layers, int hidden_dim, int 
   if (!node_feature_only) {
     ENS(ctx, ctx->feat, (size_t)LIN_ROWS * H * sizeof(float));
     float x01[2] = {0.0f, 1.0f};
-    ENS(ctx, ctx->tvals, 4096 * sizeof(float));
-    CK(ctx, cudaMemcpy(ctx->tvals.p, x01, sizeof(x01), cudaMemcpyHostToDevice));
-    k_scalar_features<<<2, H>>>((const float*)ctx->tvals.p, nullptr, ctx->dimt256, (float*)ctx->feat.p, 2);
+    CK(ctx, cudaMemcpy(ctx->tvals, x01, sizeof(x01), cudaMemcpyHostToDevice));
+    k_scalar_features<<<2, H>>>(ctx->tvals, nullptr, ctx->dimt256, (float*)ctx->feat.p, 2);
     CKL(ctx);
     k_linear<<<dim3(1, 1), 256>>>((const float*)ctx->feat.p, ctx->Wt_edge, ctx->b_edge, ctx->lut, 2, H);
     CKL(ctx);
@@ -755,9 +762,11 @@ static int run_layer(dfb_ctx* ctx, int l, float* h, float* e, const float* uv0, 
   return DFB_OK;
 }
 
-// tvec: [L][256] for this step.  binary_xt: xt in {0,1} guaranteed (categorical denoise state).
-static int run_forward(dfb_ctx* ctx, const float* xt, const float* tvec, bool binary_xt, PosteriorArgs pa,
+// Forward + head (mode HEAD_*) of step i of the staged tables: time vectors tvec[i], posterior parameters and output
+// pointers d_steps[i].  xt is the network input and the posterior's state in, xt_out its state out.
+static int run_forward(dfb_ctx* ctx, int mode, int i, const float* xt, float* xt_out, const float* uniforms,
                        cudaStream_t st) {
+  const float* tvec = (const float*)ctx->tvec.p + (size_t)i * ctx->L * H;
   const GraphDev& g = ctx->g;
   const int V = g.V, E = g.E;
   float* h = (float*)ctx->h.p;
@@ -767,7 +776,7 @@ static int run_forward(dfb_ctx* ctx, const float* xt, const float* tvec, bool bi
   if (!ctx->node_only) {
     if (!ctx->points_ready) FAIL(ctx, DFB_E_INVALID, "dfb_set_points must be called before a TSP forward");
     CK(ctx, cudaMemcpyAsync(h, ctx->h0.p, (size_t)V * H * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    if (binary_xt) {
+    if (mode == HEAD_CATEGORICAL) {   // the state is in {0,1}
       xt_lut = xt;   // layer 0 reads the 2-row LUT instead of a materialised e0
     } else {         // general values (Gaussian diffusion): e0 = edge_embed(edge_pos_embed(xt))
       const int CH = 65536;
@@ -806,14 +815,17 @@ static int run_forward(dfb_ctx* ctx, const float* xt, const float* tvec, bool bi
   k_gn_final<<<dim3(ctx->gseg.n_segs, 32), 256, 0, st>>>((const double*)ctx->gn_part.p, Z, ctx->gseg,
                                                          (float*)ctx->gn_stats.p);
   CKL(ctx);
+  const PosteriorArgs pa{mode, ctx->d_steps + i, xt, xt_out, uniforms};
   k_head<<<(R + 255) / 256, 256, 0, st>>>(Z, R, ctx->gseg, (const float*)ctx->gn_stats.p,
                                       ctx->node_only ? nullptr : g.perm, ctx->hp, pa);
   CKL(ctx);
   return DFB_OK;
 }
 
-// Pinned staging slot for this call: waits (host side) only if the copies of the call that used the slot two calls
-// ago have not executed yet, i.e. the host never runs more than one call ahead of the device.
+// One staging path for every call that runs the time MLP: stage_acquire hands out a pinned slot, the caller fills
+// h_tvals[slot][0..n) and h_steps[slot][0..n), stage_commit uploads both to tvals / d_steps and runs the time MLP of the
+// n timesteps into tvec [n][L][256].  stage_acquire waits (host side) only if the copies of the call that used the slot
+// two calls ago have not executed yet, i.e. the host never runs more than one call ahead of the device.
 static int stage_acquire(dfb_ctx* ctx, int* slot) {
   *slot = ctx->stage_next;
   ctx->stage_next = (ctx->stage_next + 1) % dfb_ctx::STAGE_SLOTS;
@@ -821,14 +833,14 @@ static int stage_acquire(dfb_ctx* ctx, int* slot) {
   return DFB_OK;
 }
 
-// all time-MLP outputs of the S timesteps staged in h_tvals[slot] -> ctx->tvec [S][L][256]
-static int compute_tvecs(dfb_ctx* ctx, int slot, int S, cudaStream_t st) {
-  ENS(ctx, ctx->tvals, std::max<size_t>(4096, (size_t)S) * sizeof(float));
-  ENS(ctx, ctx->tvec, (size_t)S * ctx->L * H * sizeof(float));
-  CK(ctx, cudaMemcpyAsync(ctx->tvals.p, ctx->h_tvals[slot], (size_t)S * sizeof(float), cudaMemcpyHostToDevice, st));
-  k_time_vectors<<<S, 256, 0, st>>>((const float*)ctx->tvals.p, ctx->tp, (const LayerParams*)ctx->layers_dev.p,
-                                    ctx->L, (float*)ctx->tvec.p);
+static int stage_commit(dfb_ctx* ctx, int slot, int n, cudaStream_t st) {
+  ENS(ctx, ctx->tvec, (size_t)n * ctx->L * H * sizeof(float));
+  CK(ctx, cudaMemcpyAsync(ctx->tvals, ctx->h_tvals[slot], (size_t)n * sizeof(float), cudaMemcpyHostToDevice, st));
+  CK(ctx, cudaMemcpyAsync(ctx->d_steps, ctx->h_steps[slot], (size_t)n * sizeof(StepParams), cudaMemcpyHostToDevice, st));
+  k_time_vectors<<<n, 256, 0, st>>>(ctx->tvals, ctx->tp, (const LayerParams*)ctx->layers_dev.p, ctx->L,
+                                    (float*)ctx->tvec.p);
   CKL(ctx);
+  CK(ctx, cudaEventRecord(ctx->stage_ev[slot], st));
   return DFB_OK;
 }
 
@@ -841,28 +853,24 @@ extern "C" int dfb_encoder_forward(dfb_ctx* ctx, const float* xt, float t, float
   int r = stage_acquire(ctx, &slot);
   if (r) return r;
   ctx->h_tvals[slot][0] = t;
-  r = compute_tvecs(ctx, slot, 1, st);
+  ctx->h_steps[slot][0] = StepParams{};
+  ctx->h_steps[slot][0].rec_out = out;
+  r = stage_commit(ctx, slot, 1, st);
   if (r) return r;
-  CK(ctx, cudaEventRecord(ctx->stage_ev[slot], st));
-  PosteriorArgs pa{};
-  pa.mode = HEAD_FORWARD;
-  pa.net_out = out;
-  return run_forward(ctx, xt, (const float*)ctx->tvec.p, false, pa, st);
+  return run_forward(ctx, HEAD_FORWARD, 0, xt, nullptr, nullptr, st);
 }
 
-static int step_args(dfb_ctx* ctx, int diffusion_type, const float* consts, int last, PosteriorArgs* pa) {
+// the head's posterior for a diffusion type, which the loaded head's out_channels must fit
+static int head_mode(dfb_ctx* ctx, int diffusion_type, int* mode) {
   if (diffusion_type == DFB_DIFFUSION_CATEGORICAL) {
     if (ctx->out_channels != 2) FAIL(ctx, DFB_E_INVALID, "categorical diffusion needs out_channels == 2");
-    pa->mode = HEAD_CATEGORICAL;
+    *mode = HEAD_CATEGORICAL;
   } else if (diffusion_type == DFB_DIFFUSION_GAUSSIAN) {
     if (ctx->out_channels != 1) FAIL(ctx, DFB_E_INVALID, "gaussian diffusion needs out_channels == 1");
-    pa->mode = HEAD_GAUSSIAN;
+    *mode = HEAD_GAUSSIAN;
   } else {
     FAIL(ctx, DFB_E_INVALID, "Unknown diffusion type %d", diffusion_type);
   }
-  if (consts)
-    for (int i = 0; i < 4; ++i) pa->c[i] = consts[i];
-  pa->last = last;
   return DFB_OK;
 }
 
@@ -873,33 +881,32 @@ extern "C" int dfb_denoise_step(dfb_ctx* ctx, int diffusion_type, const float* x
   cudaStream_t st = (cudaStream_t)stream_;
   CK(ctx, cudaSetDevice(ctx->device));
   if (!ctx->graph_ready) FAIL(ctx, DFB_E_INVALID, "dfb_prepare_graph must be called first");
-  PosteriorArgs pa{};
-  int r = step_args(ctx, diffusion_type, consts, last, &pa);
+  int mode;
+  int r = head_mode(ctx, diffusion_type, &mode);
   if (r) return r;
   int slot;
   r = stage_acquire(ctx, &slot);
   if (r) return r;
   ctx->h_tvals[slot][0] = t;
-  r = compute_tvecs(ctx, slot, 1, st);
+  StepParams& sp = ctx->h_steps[slot][0];
+  sp = StepParams{};
+  if (consts)
+    for (int k = 0; k < 4; ++k) sp.c[k] = consts[k];
+  sp.last = last;
+  sp.step = (unsigned)step_index;
+  sp.seed = seed;
+  sp.rec_out = net_out;
+  if (mode == HEAD_CATEGORICAL) sp.rec_p = p_out;   // gaussian has no p: its p_out is left untouched
+  r = stage_commit(ctx, slot, 1, st);
   if (r) return r;
-  CK(ctx, cudaEventRecord(ctx->stage_ev[slot], st));
-  pa.xt_in = xt_in; pa.uniforms = uniforms; pa.seed = seed; pa.step = (unsigned)step_index;
-  pa.xt_out = xt_out; pa.p_out = p_out; pa.net_out = net_out;
-  return run_forward(ctx, xt_in, (const float*)ctx->tvec.p, diffusion_type == DFB_DIFFUSION_CATEGORICAL, pa, st);
+  return run_forward(ctx, mode, 0, xt_in, xt_out, uniforms, st);
 }
 
 // the `steps` forwards + posteriors of the loop, every per-step quantity read from device tables
-static int enqueue_loop(dfb_ctx* ctx, int diffusion_type, float* xt, int steps, const float* uniforms, cudaStream_t st) {
+static int enqueue_loop(dfb_ctx* ctx, int mode, float* xt, int steps, const float* uniforms, cudaStream_t st) {
   const size_t N = ctx->node_only ? ctx->g.V : ctx->g.E;
   for (int i = 0; i < steps; ++i) {
-    PosteriorArgs pa{};
-    int r = step_args(ctx, diffusion_type, nullptr, 0, &pa);
-    if (r) return r;
-    pa.sp = (const StepParams*)ctx->d_steps.p + i;
-    pa.xt_in = xt; pa.xt_out = xt;
-    pa.uniforms = uniforms ? uniforms + (size_t)i * N : nullptr;
-    r = run_forward(ctx, xt, (const float*)ctx->tvec.p + (size_t)i * ctx->L * H,
-                    diffusion_type == DFB_DIFFUSION_CATEGORICAL, pa, st);
+    int r = run_forward(ctx, mode, i, xt, xt, uniforms ? uniforms + (size_t)i * N : nullptr, st);
     if (r) return r;
   }
   return DFB_OK;
@@ -922,11 +929,9 @@ extern "C" int dfb_denoise_record(dfb_ctx* ctx, int diffusion_type, float* xt, i
   if (!ctx->graph_ready) FAIL(ctx, DFB_E_INVALID, "dfb_prepare_graph must be called first");
   if (steps < 1 || steps > dfb_ctx::MAX_STEPS) FAIL(ctx, DFB_E_INVALID, "steps %d out of range", steps);
   if (!ctx->node_only && !ctx->points_ready) FAIL(ctx, DFB_E_INVALID, "dfb_set_points must be called before a TSP forward");
-  {
-    PosteriorArgs chk{};
-    int r = step_args(ctx, diffusion_type, nullptr, 0, &chk);
-    if (r) return r;
-  }
+  int mode;
+  int r = head_mode(ctx, diffusion_type, &mode);
+  if (r) return r;
   if (n_record < 0) FAIL(ctx, DFB_E_INVALID, "n_record %d < 0", n_record);
   if (n_record > 0) {
     if (!record_steps) FAIL(ctx, DFB_E_INVALID, "n_record > 0 needs record_steps");
@@ -942,7 +947,7 @@ extern "C" int dfb_denoise_record(dfb_ctx* ctx, int diffusion_type, float* xt, i
     }
   }
   int slot;
-  int r = stage_acquire(ctx, &slot);
+  r = stage_acquire(ctx, &slot);
   if (r) return r;
   const size_t N = ctx->node_only ? ctx->g.V : ctx->g.E;
   for (int i = 0, j = 0; i < steps; ++i) {
@@ -960,11 +965,8 @@ extern "C" int dfb_denoise_record(dfb_ctx* ctx, int diffusion_type, float* xt, i
       ++j;
     }
   }
-  ENS(ctx, ctx->d_steps, (size_t)dfb_ctx::MAX_STEPS * sizeof(StepParams));
-  r = compute_tvecs(ctx, slot, steps, st);
+  r = stage_commit(ctx, slot, steps, st);
   if (r) return r;
-  CK(ctx, cudaMemcpyAsync(ctx->d_steps.p, ctx->h_steps[slot], (size_t)steps * sizeof(StepParams), cudaMemcpyHostToDevice, st));
-  CK(ctx, cudaEventRecord(ctx->stage_ev[slot], st));
   // the loop state lives in the context's own buffer, so the captured graph does not depend on the caller's pointer
   float* x = (float*)ctx->d_xt.p;
   if (xt != x) CK(ctx, cudaMemcpyAsync(x, xt, N * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -983,7 +985,7 @@ extern "C" int dfb_denoise_record(dfb_ctx* ctx, int diffusion_type, float* xt, i
       cudaGraph_t graph = nullptr;
       cudaError_t ce = cudaStreamBeginCapture(ctx->loop_stream, cudaStreamCaptureModeThreadLocal);
       if (ce == cudaSuccess) {
-        r = enqueue_loop(ctx, diffusion_type, x, steps, uniforms, ctx->loop_stream);
+        r = enqueue_loop(ctx, mode, x, steps, uniforms, ctx->loop_stream);
         ce = cudaStreamEndCapture(ctx->loop_stream, &graph);
         if (r == DFB_OK && ce == cudaSuccess) ce = cudaGraphInstantiate(&ctx->loop_exec, graph, 0);
         if (graph) cudaGraphDestroy(graph);
@@ -1009,7 +1011,7 @@ extern "C" int dfb_denoise_record(dfb_ctx* ctx, int diffusion_type, float* xt, i
     CK(ctx, cudaStreamWaitEvent(st, ctx->loop_out, 0));
     ctx->launches += ctx->loop_launches;
   } else {
-    r = enqueue_loop(ctx, diffusion_type, x, steps, uniforms, st);
+    r = enqueue_loop(ctx, mode, x, steps, uniforms, st);
     if (r) return r;
   }
   if (xt != x) CK(ctx, cudaMemcpyAsync(xt, x, N * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -1108,9 +1110,9 @@ extern "C" int dfb_debug_gnn_layer(dfb_ctx* ctx, int layer, float t, float* h, f
   int r = stage_acquire(ctx, &slot);
   if (r) return r;
   ctx->h_tvals[slot][0] = t;
-  r = compute_tvecs(ctx, slot, 1, st);
+  ctx->h_steps[slot][0] = StepParams{};
+  r = stage_commit(ctx, slot, 1, st);
   if (r) return r;
-  CK(ctx, cudaEventRecord(ctx->stage_ev[slot], st));
   return run_layer(ctx, layer, h, e, nullptr, (const float*)ctx->tvec.p + (size_t)layer * H, 0, nullptr, st);
 }
 

@@ -287,43 +287,30 @@ struct HeadParams {
   int out_channels;
 };
 enum { HEAD_FORWARD = 0, HEAD_CATEGORICAL = 1, HEAD_GAUSSIAN = 2 };
-// Per-step posterior parameters in DEVICE memory: the captured CUDA graph of the denoise loop reads them through a
-// pointer, so one graph serves every schedule / seed of the same shape (only this small table is re-uploaded).
-// rec_*: this step's row of the caller's trajectory buffers (dfb_denoise_record), null when the step is not recorded;
-// living in the table, they do not make the graph depend on the caller's buffers either.
+// Per-step parameters and output pointers in DEVICE memory, one row per step: k_head's only source of them.  The
+// captured CUDA graph of the denoise loop reads its rows through a pointer, so one graph serves every schedule / seed of
+// the same shape (only this small table is re-uploaded); a single forward or step stages one row the same way.
+// rec_*: where the step writes in the caller's buffers (trajectory rows, or a single call's out / p_out / net_out), null
+// when not written; living in the table, they do not make the graph depend on the caller's buffers either.
 struct StepParams {
-  float c[4];
-  int last;
-  unsigned int step;
+  float c[4];               // categorical c[xt][k] / gaussian {a, b1, b2, noise}
+  int last;                 // categorical: target_t == 0 -> return clamp(p, min=0)
+  unsigned int step;        // Philox key (with seed)
   unsigned long long seed;
   float* rec_xt;    // (N,) state after the step
   float* rec_p;     // (N,) categorical p before sampling
   float* rec_out;   // (N, out_channels) network output
 };
+// What differs per launch of k_head besides its step's row: the state it reads and writes, and injected draws.
 struct PosteriorArgs {
-  int mode;            // HEAD_*
-  const StepParams* sp;   // when non-null, c / last / seed / step below are taken from *sp
-  float c[4];          // categorical c[xt][k] / gaussian {a, b1, b2, noise}
-  int last;            // categorical: target_t == 0 -> return clamp(p, min=0)
-  const float* xt_in;  // (N,)
-  const float* uniforms;   // (N,) or null -> Philox
-  unsigned long long seed;
-  unsigned int step;
-  float* xt_out;       // (N,)
-  float* p_out;        // optional
-  float* net_out;      // optional (N,out)
+  int mode;                 // HEAD_*
+  const StepParams* sp;     // this step's row of the device table
+  const float* xt_in;       // (N,)
+  float* xt_out;            // (N,)
+  const float* uniforms;    // (N,) or null -> Philox
 };
-__device__ __forceinline__ void head_posterior(const HeadParams& hp, const PosteriorArgs& pa_in, size_t o, float l0, float l1) {
-  PosteriorArgs pa = pa_in;
-  if (pa.sp) {
-    const StepParams& sp = *pa.sp;
-    pa.c[0] = sp.c[0]; pa.c[1] = sp.c[1]; pa.c[2] = sp.c[2]; pa.c[3] = sp.c[3];
-    pa.last = sp.last; pa.step = sp.step; pa.seed = sp.seed;
-  }
-  if (pa.net_out) {
-    pa.net_out[o * hp.out_channels] = l0;
-    if (hp.out_channels == 2) pa.net_out[o * 2 + 1] = l1;
-  }
+__device__ __forceinline__ void head_posterior(const HeadParams& hp, const PosteriorArgs& pa, size_t o, float l0, float l1) {
+  const StepParams& sp = *pa.sp;
   float p = 0.0f, res = 0.0f;
   if (pa.mode == HEAD_CATEGORICAL) {
     float m = fmaxf(l0, l1);
@@ -331,37 +318,33 @@ __device__ __forceinline__ void head_posterior(const HeadParams& hp, const Poste
     float inv = 1.0f / (e0 + e1);
     float p0 = e0 * inv, p1 = e1 * inv;
     int x = pa.xt_in[o] != 0.0f;
-    p = __fadd_rn(__fmul_rn(pa.c[2 * x], p0), __fmul_rn(pa.c[2 * x + 1], p1));
-    if (pa.p_out) pa.p_out[o] = p;
-    if (pa.last) {
+    p = __fadd_rn(__fmul_rn(sp.c[2 * x], p0), __fmul_rn(sp.c[2 * x + 1], p1));
+    if (sp.last) {
       res = fmaxf(p, 0.0f);
     } else {
-      float u = pa.uniforms ? pa.uniforms[o] : philox_uniform(pa.seed, pa.step, o);
+      float u = pa.uniforms ? pa.uniforms[o] : philox_uniform(sp.seed, sp.step, o);
       res = (u < fminf(fmaxf(p, 0.0f), 1.0f)) ? 1.0f : 0.0f;   // torch.bernoulli: 1 iff u < p
     }
     pa.xt_out[o] = res;
   } else if (pa.mode == HEAD_GAUSSIAN) {
     float x = pa.xt_in[o];
-    float y = __fmul_rn(pa.c[0], __fsub_rn(x, __fmul_rn(pa.c[1], l0)));
-    y = __fadd_rn(y, __fmul_rn(pa.c[2], l0));
-    if (pa.c[3] != 0.0f) {
-      float zn = pa.uniforms ? pa.uniforms[o] : philox_normal(pa.seed, pa.step, o);
-      y = fmaf(pa.c[3], zn, y);
+    float y = __fmul_rn(sp.c[0], __fsub_rn(x, __fmul_rn(sp.c[1], l0)));
+    y = __fadd_rn(y, __fmul_rn(sp.c[2], l0));
+    if (sp.c[3] != 0.0f) {
+      float zn = pa.uniforms ? pa.uniforms[o] : philox_normal(sp.seed, sp.step, o);
+      y = fmaf(sp.c[3], zn, y);
     }
     res = y;
     pa.xt_out[o] = res;
   }
-  // trajectory recording (dfb_denoise_record), last and through pa_in, the kernel parameter: the record pointers are
-  // then loaded only here, and k_head keeps the spills it had without them
-  if (pa_in.sp) {
-    const StepParams& sp = *pa_in.sp;
-    if (sp.rec_out) {
-      sp.rec_out[o * hp.out_channels] = l0;
-      if (hp.out_channels == 2) sp.rec_out[o * 2 + 1] = l1;
-    }
-    if (sp.rec_p) sp.rec_p[o] = p;
-    if (sp.rec_xt) sp.rec_xt[o] = res;
+  // the step's outputs, last: the rec_* pointers are then loaded only here, after the posterior math, and k_head keeps
+  // the spills it had without them
+  if (sp.rec_out) {
+    sp.rec_out[o * hp.out_channels] = l0;
+    if (hp.out_channels == 2) sp.rec_out[o * 2 + 1] = l1;
   }
+  if (sp.rec_p) sp.rec_p[o] = p;
+  if (sp.rec_xt) sp.rec_xt[o] = res;
 }
 
 // A warp takes 32 consecutive rows: lane == GroupNorm group (8 channels) for the per-row partial dot products,

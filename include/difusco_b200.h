@@ -112,7 +112,7 @@ int dfb_encoder_forward(dfb_ctx* ctx, const float* xt, float t, float* out, void
  *   uniforms     DEVICE (N,) injected U[0,1) (categorical) / N(0,1) (gaussian ddpm) draws or
  *                NULL -> in-kernel Philox4x32-10 keyed by (seed, step_index, element)
  *   xt_in/xt_out DEVICE (N,), N = E (TSP) or V (MIS); may alias
- *   p_out        DEVICE (N,) optional: pre-sampling probability p (categorical)
+ *   p_out        DEVICE (N,) optional: pre-sampling probability p (categorical; gaussian leaves it untouched)
  *   net_out      DEVICE (N,out_channels) optional: raw network output */
 int dfb_denoise_step(dfb_ctx* ctx, int diffusion_type, const float* xt_in, float t,
                      const float* consts, int last, const float* uniforms, uint64_t seed,

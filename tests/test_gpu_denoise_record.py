@@ -222,6 +222,22 @@ def test_record_matches_step_api(weights2, case):
     assert np.array_equal(xo.cpu().numpy(), r["xt"][i]), i
 
 
+def test_gaussian_step_leaves_p_out_untouched(weights2, weights1):
+  """A gaussian step has no p: dfb_denoise_step accepts a p_out and writes nothing into it."""
+  steps = 4
+  m, x0, _ = _case("gauss_ddpm", weights2, weights1, steps)
+  n = x0.size
+  _, r = _loop(m, x0, steps, [0])
+  t1s, cs, ls = _sched(m, steps)
+  xin = G.cu(x0)
+  xo, p, net = torch.empty(n, device=DEV), torch.full((n,), SENT, device=DEV), torch.empty((n, 1), device=DEV)
+  m.model.engine().denoise_step(_cabi.GAUSSIAN, xin.data_ptr(), float(t1s[0]), cs[0], ls[0], None, SEED, 0,
+                                xo.data_ptr(), p.data_ptr(), net.data_ptr(), torch.cuda.current_stream().cuda_stream)
+  torch.cuda.synchronize()
+  assert (p.cpu().numpy() == SENT).all()
+  assert np.array_equal(net.cpu().numpy(), r["out"][0]) and np.array_equal(xo.cpu().numpy(), r["xt"][0])
+
+
 # ------------------------------------------------------------------------------------------------
 # 5. every recorded step of the free-running product loop (Philox) against the fp64 oracle, no skips
 # ------------------------------------------------------------------------------------------------

@@ -17,10 +17,13 @@ AGGREGATION = {"sum": 0, "mean": 1, "max": 2}
 SYMBOLS = [
     "dfb_abi_version", "dfb_create", "dfb_destroy", "dfb_last_error", "dfb_set_aggregation",
     "dfb_set_edge_impl", "dfb_load_weights", "dfb_prepare_graph", "dfb_prepare_graph_instances", "dfb_set_points",
-    "dfb_encoder_forward", "dfb_denoise_step", "dfb_denoise", "dfb_denoise_record", "dfb_denoise_host",
+    "dfb_encoder_forward", "dfb_denoise_step", "dfb_denoise", "dfb_denoise_record", "dfb_denoise_instances",
+    "dfb_denoise_host",
     "dfb_launch_count", "dfb_profile_begin", "dfb_profile_end", "dfb_debug_edge_gemm", "dfb_debug_gnn_layer",
+    "dfb_debug_loop_captures",
     "dfb_debug_phase_cycles", "dfb_debug_watchdog", "dfb_knn_graph", "dfb_set_graph_capture",
-    "dfb_set_phase_timing", "dfb_tsp_merge_sparse", "dfb_tsp_merge_order", "dfb_two_opt", "dfb_write_heatmap_txt",
+    "dfb_set_phase_timing", "dfb_tsp_merge_sparse", "dfb_tsp_merge_order", "dfb_two_opt", "dfb_two_opt_instances",
+    "dfb_write_heatmap_txt",
 ]
 
 _lib = None
@@ -54,10 +57,14 @@ def lib():
                             C.POINTER(C.c_int32), vp, u64, vp]
   L.dfb_denoise_record.argtypes = [vp, i32, vp, i32, C.POINTER(C.c_int32), C.POINTER(f32), C.POINTER(C.c_int32), vp,
                                    u64, i32, C.POINTER(C.c_int32), vp, vp, vp, vp]
+  L.dfb_denoise_instances.argtypes = [vp, i32, vp, i32, C.POINTER(C.c_int32), C.POINTER(f32), C.POINTER(C.c_int32),
+                                      vp, i32, i32, C.POINTER(C.c_int32), vp, vp, vp, vp]
   L.dfb_denoise_host.argtypes = [vp, i32, vp, vp, i64, i64, i32, vp, i32, C.POINTER(C.c_int32),
                                  C.POINTER(f32), C.POINTER(C.c_int32), u64, vp, vp]
   L.dfb_launch_count.argtypes = [vp]
   L.dfb_launch_count.restype = i64
+  L.dfb_debug_loop_captures.argtypes = [vp]
+  L.dfb_debug_loop_captures.restype = i64
   L.dfb_profile_begin.argtypes = [vp]
   L.dfb_profile_end.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(i64)]
   L.dfb_debug_edge_gemm.argtypes = [vp, i32, vp, vp, vp]
@@ -70,6 +77,7 @@ def lib():
   L.dfb_tsp_merge_sparse.argtypes = [vp, i64, vp, vp, i64, i32, vp, C.POINTER(i64)]
   L.dfb_tsp_merge_order.argtypes = [i64, vp, i64, vp, C.POINTER(i64)]
   L.dfb_two_opt.argtypes = [vp, vp, i64, vp, i64, i64, C.POINTER(i64), vp]
+  L.dfb_two_opt_instances.argtypes = [vp, vp, vp, i64, vp, vp, i64, vp, vp]
   L.dfb_write_heatmap_txt.argtypes = [C.c_char_p, i64, vp]
   for name in SYMBOLS:
     fn = getattr(L, name)
@@ -95,6 +103,51 @@ def _raise(code, msg):
 
 
 MERGE_COMPLETE, MERGE_INCOMPLETE, MERGE_AMBIGUOUS = 0, 1, 2
+
+
+def instance_seeds_array(seeds, n_segments):
+  """instance_seeds (a sequence of Python / numpy integers in [0, 2**64), one per GroupNorm segment of the prepared
+  graph) -> uint64 numpy array.  Raises ValueError on anything else, before any device work."""
+  if isinstance(seeds, (str, bytes)) or not hasattr(seeds, "__len__"):
+    raise ValueError(f"instance_seeds must be a sequence of integers, got {type(seeds).__name__}")
+  out = []
+  for s in seeds:
+    if isinstance(s, (bool, np.bool_)) or not isinstance(s, (int, np.integer)):
+      raise ValueError(f"instance_seeds must hold integers, got {type(s).__name__}")
+    if not 0 <= int(s) < 2 ** 64:
+      raise ValueError(f"instance seed {int(s)} outside [0, 2**64)")
+    out.append(int(s))
+  if len(out) != int(n_segments):
+    raise ValueError(f"{len(out)} instance seeds for a prepared graph of {int(n_segments)} instances / samples")
+  return np.array(out, dtype=np.uint64)
+
+
+def two_opt_instances_arrays(points_list, tours_list):
+  """Per-instance points (n_i, 2) and tours (B_i, n_i + 1) -> the concatenated host arrays of dfb_two_opt_instances
+  (points (V, 2) float64, node_ptr, tour_ptr, tours int64).  Checks shapes, dtypes and sizes."""
+  if len(points_list) != len(tours_list):
+    raise ValueError(f"{len(points_list)} point sets for {len(tours_list)} tour sets")
+  if len(points_list) < 1:
+    raise ValueError("at least one instance is required")
+  pts, trs, node_ptr, tour_ptr = [], [], [0], [0]
+  for i, (p, t) in enumerate(zip(points_list, tours_list)):
+    p = np.asarray(p)
+    t = np.asarray(t)
+    if p.dtype.kind != "f" or p.ndim != 2 or p.shape[1] != 2:
+      raise ValueError(f"instance {i}: points must be a float (n, 2) array, got {p.dtype} {tuple(p.shape)}")
+    if not 3 <= p.shape[0] <= 46340:
+      raise ValueError(f"instance {i}: {p.shape[0]} nodes (must be in [3, 46340])")
+    if t.dtype.kind not in "iu" or t.ndim != 2 or t.shape[1] != p.shape[0] + 1 or t.shape[0] < 1:
+      raise ValueError(f"instance {i}: tours must be an integer (B >= 1, n + 1 = {p.shape[0] + 1}) array, got "
+                       f"{t.dtype} {tuple(t.shape)}")
+    if t.min() < 0 or t.max() >= p.shape[0]:
+      raise ValueError(f"instance {i}: tour entries must be local node ids in [0, {p.shape[0]})")
+    pts.append(np.asarray(p, np.float64))
+    trs.append(np.asarray(t, np.int64).reshape(-1))
+    node_ptr.append(node_ptr[-1] + p.shape[0])
+    tour_ptr.append(tour_ptr[-1] + t.shape[0])
+  return (np.ascontiguousarray(np.concatenate(pts)), np.array(node_ptr, np.int64), np.array(tour_ptr, np.int64),
+          np.ascontiguousarray(np.concatenate(trs)))
 
 
 def tsp_merge_sparse(points, heat, edge_index, mode=0):
@@ -246,6 +299,16 @@ class Context(object):
                                       int(seed) & 0xFFFFFFFFFFFFFFFF, n_rec, ra, rec_xt_ptr, rec_p_ptr, rec_out_ptr,
                                       stream))
 
+  def denoise_instances(self, diffusion, xt_ptr, t1, consts, last, instance_seeds_ptr, n_instances, record_steps=(),
+                        rec_xt_ptr=None, rec_p_ptr=None, rec_out_ptr=None, stream=0):
+    """denoise_record with Philox draws keyed per instance: instance_seeds_ptr is a device uint64 (n_instances,)
+    array, one seed per GroupNorm segment of the prepared graph."""
+    steps, t1a, ca, la = self._sched_arrays(t1, consts, last)
+    n_rec = len(record_steps)
+    ra = (C.c_int32 * max(n_rec, 1))(*[int(x) for x in record_steps])
+    self._ck(lib().dfb_denoise_instances(self._h, diffusion, xt_ptr, steps, t1a, ca, la, instance_seeds_ptr,
+                                         int(n_instances), n_rec, ra, rec_xt_ptr, rec_p_ptr, rec_out_ptr, stream))
+
   def denoise_host(self, diffusion, points_ptr, edge_index_ptr, num_nodes, num_edges, gn_segments, xt0_ptr,
                    t1, consts, last, seed, heatmap_ptr, stream=0):
     steps, t1a, ca, la = self._sched_arrays(t1, consts, last)
@@ -265,12 +328,31 @@ class Context(object):
                                int(max_iterations), C.byref(it), stream))
     return tours, it.value
 
+  def two_opt_instances(self, points_list, tours_list, max_iterations, stream=0):
+    """dfb_two_opt_instances: per-instance points (n_i, 2) and tours (B_i, n_i + 1) -> (list of refined tour arrays,
+    list of iteration counts); each instance as two_opt on it alone."""
+    points, node_ptr, tour_ptr, tours = two_opt_instances_arrays(points_list, tours_list)
+    its = np.zeros(len(points_list), np.int64)
+    self._ck(lib().dfb_two_opt_instances(self._h, points.ctypes.data, node_ptr.ctypes.data, len(points_list),
+                                         tour_ptr.ctypes.data, tours.ctypes.data, int(max_iterations),
+                                         its.ctypes.data, stream))
+    out, e = [], 0
+    for p, t in zip(points_list, tours_list):
+      b, n1 = np.shape(t)
+      out.append(tours[e:e + b * n1].reshape(b, n1))
+      e += b * n1
+    return out, [int(x) for x in its]
+
   def knn_graph(self, points_ptr, num_nodes, k, node_offset, edge_index_ptr, stream=0):
     self._ck(lib().dfb_knn_graph(self._h, points_ptr, int(num_nodes), int(k), int(node_offset), edge_index_ptr, stream))
 
   # ---- accounting ----
   def launch_count(self):
     return int(lib().dfb_launch_count(self._h))
+
+  def loop_captures(self):
+    """How many times the denoise loop has been captured into a CUDA graph on this context."""
+    return int(lib().dfb_debug_loop_captures(self._h))
 
   def profile_begin(self):
     self._ck(lib().dfb_profile_begin(self._h))

@@ -53,10 +53,10 @@ struct dfb_ctx {
   GraphDev g{};
   GnSegments gseg{};      // head GroupNorm segments (kernels_small.cuh)
   int gn_blocks = 0;      // k_gn_partial blocks over all segments
-  DevBuf d_row, d_col, d_perm, d_rowptr, d_grp_first, d_grp_pair, d_ei_stage, d_seg_start, d_seg_blk_first, d_gn_blk;
+  DevBuf d_row, d_col, d_perm, d_rowptr, d_grp_first, d_grp_pair, d_ei_stage, d_seg_start, d_seg_blk_first, d_gn_blk, d_local;
   // ---- workspace ----
   DevBuf e, h, h0, uvab, uvab0, partials, feat, tvec, gn_part, gn_stats, d_points, d_xt, d_u;
-  DevBuf opt_points, opt_tours, opt_pos, opt_dnext, opt_cand, opt_tiles, opt_state, opt_best;   // 2-opt (row f3)
+  DevBuf opt_points, opt_tours, opt_pos, opt_dnext, opt_cand, opt_tiles, opt_state, opt_best, opt_inst, opt_tour_inst;   // 2-opt (row f3)
   // ---- step staging (pinned) + captured loop ----
   // dfb_denoise_step / dfb_denoise never allocate, never synchronise the host with the stream and never touch the
   // heap after the first call of a shape: timesteps and per-step parameters go through two pinned staging slots
@@ -86,6 +86,7 @@ struct dfb_ctx {
     }
   } loop_key;
   int64_t loop_launches = 0;     // kernel launches inside one replay of the captured loop
+  int64_t loop_captures = 0;     // successful captures of the loop (dfb_debug_loop_captures)
   // ---- accounting ----
   int64_t launches = 0;
   bool profiling = false;
@@ -542,6 +543,10 @@ static int prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_t V64, i
   const int nb = (int)gn_blk.size();
 
   std::vector<int> row(E), col(E), perm;
+  // the rank of each head row's element among its segment's elements in caller order (GnSegments::local): needed only
+  // when the sort moved edges and there is more than one segment
+  std::vector<int> local;
+  if (!sorted && !ctx->node_only && S > 1) local.resize(E);
   if (sorted) {
     for (int s = 0; s < E; ++s) {
       row[s] = (int)row64[s];
@@ -550,11 +555,13 @@ static int prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_t V64, i
   } else {   // stable counting sort by row
     perm.resize(E);
     std::vector<int> cur(rowptr.begin(), rowptr.end() - 1);
+    std::vector<int> seen(local.empty() ? 0 : S, 0);
     for (int s = 0; s < E; ++s) {
       int pos = cur[row64[s]]++;
       perm[pos] = s;
       row[pos] = (int)row64[s];
       col[pos] = (int)col64[s];
+      if (!local.empty()) local[pos] = seen[node_ptr ? inst[row64[s]] : (int)((int64_t)pos / (R / S))]++;
     }
   }
   const int nG = (E + GROUP - 1) / GROUP;
@@ -588,6 +595,10 @@ static int prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_t V64, i
   CK(ctx, cudaMemcpyAsync(ctx->d_seg_start.p, seg_start.data(), ((size_t)S + 1) * 4, cudaMemcpyHostToDevice, st));
   CK(ctx, cudaMemcpyAsync(ctx->d_seg_blk_first.p, blk_first.data(), ((size_t)S + 1) * 4, cudaMemcpyHostToDevice, st));
   CK(ctx, cudaMemcpyAsync(ctx->d_gn_blk.p, gn_blk.data(), (size_t)nb * sizeof(int2), cudaMemcpyHostToDevice, st));
+  if (!local.empty()) {
+    ENS(ctx, ctx->d_local, (size_t)E * 4);
+    CK(ctx, cudaMemcpyAsync(ctx->d_local.p, local.data(), (size_t)E * 4, cudaMemcpyHostToDevice, st));
+  }
   CK(ctx, cudaStreamSynchronize(st));   // host vectors go out of scope
   GraphDev& g = ctx->g;
   g.V = V; g.E = E;
@@ -600,6 +611,7 @@ static int prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_t V64, i
   ctx->gseg.start = (const int*)ctx->d_seg_start.p;
   ctx->gseg.blk_first = (const int*)ctx->d_seg_blk_first.p;
   ctx->gseg.blk = (const int2*)ctx->d_gn_blk.p;
+  ctx->gseg.local = local.empty() ? nullptr : (const int*)ctx->d_local.p;
   ctx->gn_blocks = nb;
 
   // workspace
@@ -816,7 +828,7 @@ static int run_forward(dfb_ctx* ctx, int mode, int i, const float* xt, float* xt
                                                          (float*)ctx->gn_stats.p);
   CKL(ctx);
   const PosteriorArgs pa{mode, ctx->d_steps + i, xt, xt_out, uniforms};
-  k_head<<<(R + 255) / 256, 256, 0, st>>>(Z, R, ctx->gseg, (const float*)ctx->gn_stats.p,
+  k_head<<<(R + HEAD_THREADS - 1) / HEAD_THREADS, HEAD_THREADS, 0, st>>>(Z, R, ctx->gseg, (const float*)ctx->gn_stats.p,
                                       ctx->node_only ? nullptr : g.perm, ctx->hp, pa);
   CKL(ctx);
   return DFB_OK;
@@ -919,14 +931,12 @@ extern "C" int dfb_denoise(dfb_ctx* ctx, int diffusion_type, float* xt, int step
                             nullptr, nullptr, nullptr, stream_);
 }
 
-extern "C" int dfb_denoise_record(dfb_ctx* ctx, int diffusion_type, float* xt, int steps, const int32_t* t1,
-                                  const float* consts, const int32_t* last_flags, const float* uniforms,
-                                  uint64_t seed, int n_record, const int32_t* record_steps, float* rec_xt,
-                                  float* rec_p, float* rec_out, void* stream_) {
-  if (!ctx) return DFB_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream_;
-  CK(ctx, cudaSetDevice(ctx->device));
-  if (!ctx->graph_ready) FAIL(ctx, DFB_E_INVALID, "dfb_prepare_graph must be called first");
+// The loop of dfb_denoise_record and dfb_denoise_instances: every argument is checked before any device work.
+// inst_seeds (DEVICE, one per segment) non-null selects per-instance keying, travelling in every step's row.
+static int denoise_loop(dfb_ctx* ctx, int diffusion_type, float* xt, int steps, const int32_t* t1, const float* consts,
+                        const int32_t* last_flags, const float* uniforms, uint64_t seed, const uint64_t* inst_seeds,
+                        int n_record, const int32_t* record_steps, float* rec_xt, float* rec_p, float* rec_out,
+                        cudaStream_t st) {
   if (steps < 1 || steps > dfb_ctx::MAX_STEPS) FAIL(ctx, DFB_E_INVALID, "steps %d out of range", steps);
   if (!ctx->node_only && !ctx->points_ready) FAIL(ctx, DFB_E_INVALID, "dfb_set_points must be called before a TSP forward");
   int mode;
@@ -957,6 +967,7 @@ extern "C" int dfb_denoise_record(dfb_ctx* ctx, int diffusion_type, float* xt, i
     sp.last = last_flags[i];
     sp.step = (unsigned)i;
     sp.seed = seed;
+    sp.inst_seeds = (const unsigned long long*)inst_seeds;
     sp.rec_xt = sp.rec_p = sp.rec_out = nullptr;
     if (j < n_record && record_steps[j] == i) {
       if (rec_xt) sp.rec_xt = rec_xt + (size_t)j * N;
@@ -1000,6 +1011,7 @@ extern "C" int dfb_denoise_record(dfb_ctx* ctx, int diffusion_type, float* xt, i
         if (r != DFB_OK) return r;
       } else {
         ctx->loop_key = key;
+        ctx->loop_captures++;
       }
     }
   }
@@ -1016,6 +1028,33 @@ extern "C" int dfb_denoise_record(dfb_ctx* ctx, int diffusion_type, float* xt, i
   }
   if (xt != x) CK(ctx, cudaMemcpyAsync(xt, x, N * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return DFB_OK;
+}
+
+extern "C" int dfb_denoise_record(dfb_ctx* ctx, int diffusion_type, float* xt, int steps, const int32_t* t1,
+                                  const float* consts, const int32_t* last_flags, const float* uniforms,
+                                  uint64_t seed, int n_record, const int32_t* record_steps, float* rec_xt,
+                                  float* rec_p, float* rec_out, void* stream_) {
+  if (!ctx) return DFB_E_INVALID;
+  CK(ctx, cudaSetDevice(ctx->device));
+  if (!ctx->graph_ready) FAIL(ctx, DFB_E_INVALID, "dfb_prepare_graph must be called first");
+  return denoise_loop(ctx, diffusion_type, xt, steps, t1, consts, last_flags, uniforms, seed, nullptr, n_record,
+                      record_steps, rec_xt, rec_p, rec_out, (cudaStream_t)stream_);
+}
+
+extern "C" int dfb_denoise_instances(dfb_ctx* ctx, int diffusion_type, float* xt, int steps, const int32_t* t1,
+                                     const float* consts, const int32_t* last_flags, const uint64_t* instance_seeds,
+                                     int n_instances, int n_record, const int32_t* record_steps, float* rec_xt,
+                                     float* rec_p, float* rec_out, void* stream_) {
+  if (!ctx) return DFB_E_INVALID;
+  CK(ctx, cudaSetDevice(ctx->device));
+  if (!ctx->graph_ready) FAIL(ctx, DFB_E_INVALID, "dfb_prepare_graph must be called first");
+  if (!instance_seeds) FAIL(ctx, DFB_E_INVALID, "instance_seeds is required");
+  if (!is_device_ptr(instance_seeds)) FAIL(ctx, DFB_E_INVALID, "instance_seeds must be a device pointer");
+  if (n_instances != ctx->gseg.n_segs)
+    FAIL(ctx, DFB_E_INVALID, "%d instance seeds for a prepared graph of %d GroupNorm segments", n_instances,
+         ctx->gseg.n_segs);
+  return denoise_loop(ctx, diffusion_type, xt, steps, t1, consts, last_flags, nullptr, 0, instance_seeds, n_record,
+                      record_steps, rec_xt, rec_p, rec_out, (cudaStream_t)stream_);
 }
 
 extern "C" int dfb_set_graph_capture(dfb_ctx* ctx, int enabled) {
@@ -1095,6 +1134,8 @@ extern "C" int dfb_debug_edge_gemm(dfb_ctx* ctx, int layer, const float* e_in, f
   ctx->launches++;
   return DFB_OK;
 }
+
+extern "C" int64_t dfb_debug_loop_captures(const dfb_ctx* ctx) { return ctx ? ctx->loop_captures : 0; }
 
 // Test hook: GNN layer `layer` alone (run_layer, the code run_forward runs for it) at timestep t, in place on the
 // caller's h (V,256) and e (E,256, row-sorted).  Always reads e and computes the node linears of h: never the LUT,
@@ -1244,6 +1285,125 @@ extern "C" int dfb_two_opt(dfb_ctx* ctx, const double* points, int64_t n, int64_
   CK(ctx, cudaMemcpyAsync(tours, d_tours, (size_t)B * (N + 1) * sizeof(long long), cudaMemcpyDeviceToHost, st));
   CK(ctx, cudaStreamSynchronize(st));
   *iterations_out = hs.iterations;
+  return DFB_OK;
+}
+
+// dfb_two_opt over many instances at once: one work list of (instance, tour, tile) for the eval kernel, one apply block
+// per instance, every instance under its own stopping rule and cap.  Each instance's tours and iterations are those of
+// dfb_two_opt on it alone: the same tiles, candidates and reductions from per-instance base offsets.
+extern "C" int dfb_two_opt_instances(dfb_ctx* ctx, const double* points, const int64_t* node_ptr, int64_t n_instances,
+                                     const int64_t* tour_ptr, int64_t* tours, int64_t max_iterations,
+                                     int64_t* iterations_out, void* stream_) {
+  if (!ctx) return DFB_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream_;
+  CK(ctx, cudaSetDevice(ctx->device));
+  if (!points || !node_ptr || !tour_ptr || !tours || !iterations_out) FAIL(ctx, DFB_E_INVALID, "two_opt_instances: null argument");
+  if (n_instances < 1 || n_instances > 0x7fffffff)
+    FAIL(ctx, DFB_E_INVALID, "two_opt_instances: n_instances %lld out of range", (long long)n_instances);
+  if (node_ptr[0] != 0 || tour_ptr[0] != 0) FAIL(ctx, DFB_E_INVALID, "two_opt_instances: node_ptr and tour_ptr must start at 0");
+  const int NI = (int)n_instances;
+  std::vector<TwoOptInst> insts(NI);
+  std::vector<TwoOptState> states(NI);
+  int64_t entries = 0, items = 0;
+  for (int i = 0; i < NI; ++i) {
+    const int64_t n = node_ptr[i + 1] - node_ptr[i], B = tour_ptr[i + 1] - tour_ptr[i];
+    if (n < 3 || n > 46340) FAIL(ctx, DFB_E_INVALID, "two_opt_instances: instance %d has %lld nodes (must be in [3, 46340])", i, (long long)n);
+    if (B < 1) FAIL(ctx, DFB_E_INVALID, "two_opt_instances: instance %d has %lld tours (at least 1)", i, (long long)B);
+    if (node_ptr[i + 1] > 0x7fffffff || tour_ptr[i + 1] > 0x7fffffff)
+      FAIL(ctx, DFB_E_INVALID, "two_opt_instances: more than 2^31 - 1 nodes or tours");
+    const int T = (int)((n + TWOOPT_TILE - 1) / TWOOPT_TILE);
+    TwoOptInst& in = insts[i];
+    in.tour0 = entries;
+    in.dnext0 = entries - tour_ptr[i];
+    in.cand0 = items;
+    in.node0 = (int)node_ptr[i];
+    in.n = (int)n;
+    in.B = (int)B;
+    in.ntiles = T * (T + 1) / 2;
+    in.tour_first = (int)tour_ptr[i];
+    entries += B * (n + 1);
+    items += B * in.ntiles;
+    if (items > 0x7fffffff) FAIL(ctx, DFB_E_INVALID, "two_opt_instances: more than 2^31 - 1 eval tiles in one call");
+  }
+  int running = 0;
+  for (int i = 0; i < NI; ++i) {
+    const TwoOptInst& in = insts[i];
+    const double* p = points + 2 * (int64_t)in.node0;
+    bool finite = true;
+    for (int64_t k = in.tour0; k < in.tour0 + (int64_t)in.B * (in.n + 1); ++k) {
+      if (tours[k] < 0 || tours[k] >= in.n)
+        FAIL(ctx, DFB_E_INVALID, "two_opt_instances: instance %d: tour entry %lld out of range", i, (long long)tours[k]);
+      finite = finite && std::isfinite(p[2 * tours[k]]) && std::isfinite(p[2 * tours[k] + 1]);
+    }
+    // as in dfb_two_opt: a non-finite point on a tour leaves the instance's tours unchanged after 0 iterations
+    states[i] = TwoOptState{finite ? 0 : 1, 0, 0};
+    running += finite;
+  }
+  if (running == 0) {
+    for (int i = 0; i < NI; ++i) iterations_out[i] = 0;
+    return DFB_OK;
+  }
+  const int n_tours = (int)tour_ptr[NI];
+  const int64_t V = node_ptr[NI];
+  std::vector<TwoOptWork> work((size_t)items);
+  std::vector<int> tour_inst(n_tours);
+  for (int i = 0; i < NI; ++i) {
+    const TwoOptInst& in = insts[i];
+    const int T = (in.n + TWOOPT_TILE - 1) / TWOOPT_TILE;
+    int64_t w = in.cand0;
+    for (int b = 0; b < in.B; ++b) {
+      tour_inst[in.tour_first + b] = i;
+      for (int a = 0; a < T; ++a)   // dfb_two_opt's tile order
+        for (int c = a; c < T; ++c) work[w++] = TwoOptWork{i, b, a, c};
+    }
+  }
+  ENS(ctx, ctx->opt_points, (size_t)V * 2 * sizeof(double));
+  ENS(ctx, ctx->opt_tours, (size_t)entries * sizeof(long long));
+  ENS(ctx, ctx->opt_pos, (size_t)entries * 2 * sizeof(double));
+  ENS(ctx, ctx->opt_dnext, (size_t)(entries - n_tours) * sizeof(double));
+  ENS(ctx, ctx->opt_cand, (size_t)items * sizeof(TwoOptCand));
+  ENS(ctx, ctx->opt_tiles, (size_t)items * sizeof(TwoOptWork));
+  ENS(ctx, ctx->opt_state, (size_t)NI * sizeof(TwoOptState) + sizeof(int));
+  ENS(ctx, ctx->opt_best, (size_t)n_tours * sizeof(TwoOptCand));
+  ENS(ctx, ctx->opt_inst, (size_t)NI * sizeof(TwoOptInst));
+  ENS(ctx, ctx->opt_tour_inst, (size_t)n_tours * sizeof(int));
+  double* d_points = (double*)ctx->opt_points.p;
+  long long* d_tours = (long long*)ctx->opt_tours.p;
+  double* d_pos = (double*)ctx->opt_pos.p;
+  double* d_dnext = (double*)ctx->opt_dnext.p;
+  TwoOptCand* d_cand = (TwoOptCand*)ctx->opt_cand.p;
+  TwoOptWork* d_work = (TwoOptWork*)ctx->opt_tiles.p;
+  TwoOptState* d_states = (TwoOptState*)ctx->opt_state.p;
+  int* d_running = (int*)(d_states + NI);
+  TwoOptInst* d_insts = (TwoOptInst*)ctx->opt_inst.p;
+  int* d_tour_inst = (int*)ctx->opt_tour_inst.p;
+  CK(ctx, cudaMemcpyAsync(d_points, points, (size_t)V * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(ctx, cudaMemcpyAsync(d_tours, tours, (size_t)entries * sizeof(long long), cudaMemcpyHostToDevice, st));
+  CK(ctx, cudaMemcpyAsync(d_work, work.data(), (size_t)items * sizeof(TwoOptWork), cudaMemcpyHostToDevice, st));
+  CK(ctx, cudaMemcpyAsync(d_states, states.data(), (size_t)NI * sizeof(TwoOptState), cudaMemcpyHostToDevice, st));
+  CK(ctx, cudaMemcpyAsync(d_running, &running, sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(ctx, cudaMemcpyAsync(d_insts, insts.data(), (size_t)NI * sizeof(TwoOptInst), cudaMemcpyHostToDevice, st));
+  CK(ctx, cudaMemcpyAsync(d_tour_inst, tour_inst.data(), (size_t)n_tours * sizeof(int), cudaMemcpyHostToDevice, st));
+  k_twoopt_init_instances<<<n_tours, 256, 0, st>>>(d_points, d_tours, d_pos, d_dnext, d_insts, d_tour_inst);
+  CKL(ctx);
+  int chunk = 8;
+  while (true) {
+    for (int c = 0; c < chunk; ++c) {
+      k_twoopt_eval_instances<<<(unsigned)items, 256, 0, st>>>(d_pos, d_dnext, d_insts, d_work, d_cand, d_states);
+      CKL(ctx);
+      k_twoopt_apply_instances<<<NI, 1024, 0, st>>>(d_tours, d_pos, d_dnext, d_cand, d_insts, d_states,
+                                                     (TwoOptCand*)ctx->opt_best.p, d_running, (long long)max_iterations);
+      CKL(ctx);
+    }
+    CK(ctx, cudaMemcpyAsync(&running, d_running, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaStreamSynchronize(st));
+    if (running == 0) break;
+    if (chunk < 64) chunk *= 2;
+  }
+  CK(ctx, cudaMemcpyAsync(tours, d_tours, (size_t)entries * sizeof(long long), cudaMemcpyDeviceToHost, st));
+  CK(ctx, cudaMemcpyAsync(states.data(), d_states, (size_t)NI * sizeof(TwoOptState), cudaMemcpyDeviceToHost, st));
+  CK(ctx, cudaStreamSynchronize(st));
+  for (int i = 0; i < NI; ++i) iterations_out[i] = states[i].iterations;
   return DFB_OK;
 }
 

@@ -208,6 +208,10 @@ struct GnSegments {
   const int* start;       // [n_segs + 1] first head row of each segment; start[n_segs] = rows of the call
   const int* blk_first;   // [n_segs + 1] first k_gn_partial block of each segment; blk_first[n_segs] = block count
   const int2* blk;        // [block count] {segment, first row}: GN_ROWS_PER_BLOCK rows counted from the segment's start
+  // [rows] or null: the rank of head row r's element among its segment's elements in the caller's order (the Philox
+  // element index of per-instance keying).  Built only when the rows are a permutation of the caller's elements and
+  // there is more than one segment; otherwise that rank is the caller index minus the segment's first row.
+  const int* local;
 };
 __device__ __forceinline__ float gn_pivot(const float* Z, int seg_row0, int group) {
   return Z[(size_t)seg_row0 * H + group * 8];
@@ -300,6 +304,10 @@ struct StepParams {
   float* rec_xt;    // (N,) state after the step
   float* rec_p;     // (N,) categorical p before sampling
   float* rec_out;   // (N, out_channels) network output
+  // (segments,) or null: per-instance keying (dfb_denoise_instances).  The element of head row r is then drawn with
+  // (inst_seeds[s], step, rank of the element among segment s's elements in caller order), s the segment of r: what the
+  // instance alone, with that seed, draws for it.  Null: (seed, step, caller index), keyed by the whole call.
+  const unsigned long long* inst_seeds;
 };
 // What differs per launch of k_head besides its step's row: the state it reads and writes, and injected draws.
 struct PosteriorArgs {
@@ -309,8 +317,21 @@ struct PosteriorArgs {
   float* xt_out;            // (N,)
   const float* uniforms;    // (N,) or null -> Philox
 };
-__device__ __forceinline__ void head_posterior(const HeadParams& hp, const PosteriorArgs& pa, size_t o, float l0, float l1) {
+__device__ __forceinline__ void head_posterior(const HeadParams& hp, const PosteriorArgs& pa, const GnSegments& sg,
+                                               int r, size_t o, float l0, float l1) {
   const StepParams& sp = *pa.sp;
+  // Philox key of the element: (seed, caller index o), or per instance (see StepParams::inst_seeds) the seed of row r's
+  // segment and the element's rank among that segment's elements
+  unsigned long long seed = sp.seed, elem = o;
+  if (sp.inst_seeds) {
+    int s = 0;
+    for (int hi = sg.n_segs; hi - s > 1;) {
+      const int mid = (s + hi) >> 1;
+      if (sg.start[mid] <= r) s = mid; else hi = mid;
+    }
+    seed = sp.inst_seeds[s];
+    elem = sg.local ? (unsigned long long)sg.local[r] : (unsigned long long)(o - (size_t)sg.start[s]);
+  }
   float p = 0.0f, res = 0.0f;
   if (pa.mode == HEAD_CATEGORICAL) {
     float m = fmaxf(l0, l1);
@@ -322,7 +343,7 @@ __device__ __forceinline__ void head_posterior(const HeadParams& hp, const Poste
     if (sp.last) {
       res = fmaxf(p, 0.0f);
     } else {
-      float u = pa.uniforms ? pa.uniforms[o] : philox_uniform(sp.seed, sp.step, o);
+      float u = pa.uniforms ? pa.uniforms[o] : philox_uniform(seed, sp.step, elem);
       res = (u < fminf(fmaxf(p, 0.0f), 1.0f)) ? 1.0f : 0.0f;   // torch.bernoulli: 1 iff u < p
     }
     pa.xt_out[o] = res;
@@ -331,7 +352,7 @@ __device__ __forceinline__ void head_posterior(const HeadParams& hp, const Poste
     float y = __fmul_rn(sp.c[0], __fsub_rn(x, __fmul_rn(sp.c[1], l0)));
     y = __fadd_rn(y, __fmul_rn(sp.c[2], l0));
     if (sp.c[3] != 0.0f) {
-      float zn = pa.uniforms ? pa.uniforms[o] : philox_normal(sp.seed, sp.step, o);
+      float zn = pa.uniforms ? pa.uniforms[o] : philox_normal(seed, sp.step, elem);
       y = fmaf(sp.c[3], zn, y);
     }
     res = y;
@@ -347,15 +368,17 @@ __device__ __forceinline__ void head_posterior(const HeadParams& hp, const Poste
   if (sp.rec_xt) sp.rec_xt[o] = res;
 }
 
+// Block size of k_head: its launch, its launch bounds and its row index all use this one constant.
+constexpr int HEAD_THREADS = 256;
 // A warp takes 32 consecutive rows: lane == GroupNorm group (8 channels) for the per-row partial dot products,
 // then a butterfly transpose-reduce (31 shuffles per output channel for all 32 rows) leaves row j's logits in
 // lane j, so the softmax / posterior / Philox epilogue runs on all 32 lanes in parallel.
-__global__ void __launch_bounds__(256, 2) k_head(const float* __restrict__ Z, int R, GnSegments sg,
+__global__ void __launch_bounds__(HEAD_THREADS, 2) k_head(const float* __restrict__ Z, int R, GnSegments sg,
                                               const float* __restrict__ stats,
                                               const int* __restrict__ perm, HeadParams hp,
                                               PosteriorArgs pa) {
   const int lane = threadIdx.x & 31;
-  const int warp_global = blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int warp_global = blockIdx.x * (HEAD_THREADS / 32) + (threadIdx.x >> 5);
   const int r0 = warp_global * 32;
   if (r0 >= R) return;
   float g[8], b[8], w0[8], w1[8];
@@ -412,10 +435,15 @@ __global__ void __launch_bounds__(256, 2) k_head(const float* __restrict__ Z, in
       a1[i] = k1 + __shfl_xor_sync(0xffffffffu, s1, off);
     }
   }
-  const int r = r0 + lane;
+  // r0 + lane, re-read from the special registers: held from the kernel's start, the row index costs k_head a spill
+  // once the per-instance Philox key needs it after the posterior
+  unsigned int bx, tx;
+  asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(bx));
+  asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tx));
+  const int r = (int)(bx * HEAD_THREADS + tx);
   if (r >= R) return;
   const size_t o = perm ? (size_t)perm[r] : (size_t)r;
-  head_posterior(hp, pa, o, a0[0] + hp.b[0], (hp.out_channels == 2) ? a1[0] + hp.b[1] : 0.0f);
+  head_posterior(hp, pa, sg, r, o, a0[0] + hp.b[0], (hp.out_channels == 2) ? a1[0] + hp.b[1] : 0.0f);
 }
 
 }  // namespace dfb

@@ -237,37 +237,65 @@ __device__ __forceinline__ double twoopt_dist(double ax, double ay, double bx, d
   return __dsqrt_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)));
 }
 
-// pos (B, N+1, 2): coordinates along the tour; dnext (B, N): |pos[k] - pos[k+1]|.
-__global__ void k_twoopt_init(const double* __restrict__ points, const long long* __restrict__ tours, double* __restrict__ pos,
-                              double* __restrict__ dnext, int N) {
-  const int b = blockIdx.y;
-  const long long* tour = tours + (size_t)b * (N + 1);
-  double* P = pos + (size_t)b * (N + 1) * 2;
-  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k <= N; k += gridDim.x * blockDim.x) {
+// Per instance of dfb_two_opt_instances: where its tours start in the concatenated buffers and its shape.  Its B tours of
+// n + 1 entries are consecutive, so from these bases on the instance is exactly one dfb_two_opt problem.
+struct TwoOptInst {
+  long long tour0;    // first entry of its first tour in tours (pos: 2 x)
+  long long dnext0;   // first entry in dnext (n per tour)
+  long long cand0;    // first candidate slot (= first work item; ntiles per tour)
+  int node0;          // first node in points
+  int n, B, ntiles;
+  int tour_first;     // global index of its first tour (slot in the per-tour arg-min array)
+};
+// One eval block of dfb_two_opt_instances: instance, its tour, and the tile (a, b).  The list is instance-major, then tour,
+// then tile, so an instance's candidates have dfb_two_opt's layout from TwoOptInst::cand0 on.
+struct TwoOptWork {
+  int inst, tour, a, b;
+};
+
+// One tour's pos (N+1, 2) and dnext (N): coordinates along the tour and |pos[k] - pos[k+1]|.  Entries k0, k0 + stride, ...
+__device__ __forceinline__ void twoopt_init_tour(const double* __restrict__ points, const long long* __restrict__ tour,
+                                                 double* __restrict__ P, double* __restrict__ D, int N, int k0, int stride) {
+  for (int k = k0; k <= N; k += stride) {
     long long v = tour[k];
     P[2 * k] = points[2 * v];
     P[2 * k + 1] = points[2 * v + 1];
   }
-  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < N; k += gridDim.x * blockDim.x) {
+  for (int k = k0; k < N; k += stride) {
     long long v = tour[k], w = tour[k + 1];
-    dnext[(size_t)b * N + k] = twoopt_dist(points[2 * v], points[2 * v + 1], points[2 * w], points[2 * w + 1]);
+    D[k] = twoopt_dist(points[2 * v], points[2 * v + 1], points[2 * w], points[2 * w + 1]);
   }
 }
 
-// One 64x64 tile of moves (i in tile row, j in tile column, j >= i + 2) per block; grid (tiles, B).
+// pos (B, N+1, 2): coordinates along the tour; dnext (B, N): |pos[k] - pos[k+1]|.
+__global__ void k_twoopt_init(const double* __restrict__ points, const long long* __restrict__ tours, double* __restrict__ pos,
+                              double* __restrict__ dnext, int N) {
+  const int b = blockIdx.y;
+  twoopt_init_tour(points, tours + (size_t)b * (N + 1), pos + (size_t)b * (N + 1) * 2, dnext + (size_t)b * N, N,
+                   blockIdx.x * blockDim.x + threadIdx.x, gridDim.x * blockDim.x);
+}
+
+// One block per tour of every instance.
+__global__ void k_twoopt_init_instances(const double* __restrict__ points, const long long* __restrict__ tours,
+                                        double* __restrict__ pos, double* __restrict__ dnext,
+                                        const TwoOptInst* __restrict__ insts, const int* __restrict__ tour_inst) {
+  const TwoOptInst in = insts[tour_inst[blockIdx.x]];
+  const long long t = blockIdx.x - in.tour_first;
+  const long long e0 = in.tour0 + t * (in.n + 1);
+  twoopt_init_tour(points + 2 * (size_t)in.node0, tours + e0, pos + 2 * e0, dnext + in.dnext0 + t * in.n, in.n,
+                   threadIdx.x, blockDim.x);
+}
+
+// The best move of one 64x64 tile (i in tile row t.x, j in tile column t.y, j >= i + 2) of one tour, by one block of 256
+// threads, into *out.  P, D: the tour's pos and dnext.
 //   change(i, j) = ((|p_i - p_j| + |p_i+1 - p_j+1|) - |p_i - p_i+1|) - |p_j - p_j+1|      tsp_utils.py:21-31
-__global__ void __launch_bounds__(256) k_twoopt_eval(const double* __restrict__ pos, const double* __restrict__ dnext,
-                                                     const int2* __restrict__ tiles, TwoOptCand* __restrict__ cand,
-                                                     const TwoOptState* __restrict__ state, int N, int ntiles) {
-  if (state->done) return;
+__device__ __forceinline__ void twoopt_eval_tile(const double* __restrict__ P, const double* __restrict__ D, int2 t, int N,
+                                                 TwoOptCand* __restrict__ out) {
   __shared__ double s_ix[TWOOPT_TILE + 1], s_iy[TWOOPT_TILE + 1], s_jx[TWOOPT_TILE + 1], s_jy[TWOOPT_TILE + 1];
   __shared__ double s_di[TWOOPT_TILE], s_dj[TWOOPT_TILE];
   __shared__ TwoOptCand s_red[8];
-  const int b = blockIdx.y, tid = threadIdx.x;
-  const int2 t = tiles[blockIdx.x];
+  const int tid = threadIdx.x;
   const int i0 = t.x * TWOOPT_TILE, j0 = t.y * TWOOPT_TILE;
-  const double* P = pos + (size_t)b * (N + 1) * 2;
-  const double* D = dnext + (size_t)b * N;
   if (tid <= TWOOPT_TILE) {
     int k = min(i0 + tid, N);
     s_ix[tid] = P[2 * k];
@@ -320,17 +348,42 @@ __global__ void __launch_bounds__(256) k_twoopt_eval(const double* __restrict__ 
         best = s_red[w].val;
         bidx = s_red[w].idx;
       }
-    cand[(size_t)b * ntiles + blockIdx.x] = {best, bidx};
+    *out = {best, bidx};
   }
 }
 
-// Single block: reduce the tile candidates of every tour, take the batch-wide minimum for the stopping rule
-// (tsp_utils.py:33, :39, :44-48), reverse tour[min_i+1 .. min_j] of EVERY tour (the reference applies each tour's
-// own arg-min whenever the batch minimum passes the threshold), refresh dnext.
-__global__ void __launch_bounds__(1024) k_twoopt_apply(long long* __restrict__ tours, double* __restrict__ pos,
-                                                       double* __restrict__ dnext, const TwoOptCand* __restrict__ cand,
-                                                       TwoOptState* __restrict__ state, TwoOptCand* __restrict__ s_best,
-                                                       int N, int B, int ntiles, long long max_iterations) {
+// grid (tiles, B)
+__global__ void __launch_bounds__(256) k_twoopt_eval(const double* __restrict__ pos, const double* __restrict__ dnext,
+                                                     const int2* __restrict__ tiles, TwoOptCand* __restrict__ cand,
+                                                     const TwoOptState* __restrict__ state, int N, int ntiles) {
+  if (state->done) return;
+  const int b = blockIdx.y;
+  twoopt_eval_tile(pos + (size_t)b * (N + 1) * 2, dnext + (size_t)b * N, tiles[blockIdx.x], N,
+                   cand + (size_t)b * ntiles + blockIdx.x);
+}
+
+// One block per work item of every instance; the blocks of a finished instance return at once.
+__global__ void __launch_bounds__(256) k_twoopt_eval_instances(const double* __restrict__ pos,
+                                                               const double* __restrict__ dnext,
+                                                               const TwoOptInst* __restrict__ insts,
+                                                               const TwoOptWork* __restrict__ work,
+                                                               TwoOptCand* __restrict__ cand,
+                                                               const TwoOptState* __restrict__ states) {
+  const TwoOptWork w = work[blockIdx.x];
+  if (states[w.inst].done) return;
+  const TwoOptInst in = insts[w.inst];
+  const long long e0 = in.tour0 + (long long)w.tour * (in.n + 1);
+  twoopt_eval_tile(pos + 2 * e0, dnext + in.dnext0 + (long long)w.tour * in.n, make_int2(w.a, w.b), in.n,
+                   cand + blockIdx.x);
+}
+
+// One iteration of one batch of B tours, by one block of 1024 threads: reduce the tile candidates of every tour, take the
+// batch-wide minimum for the stopping rule (tsp_utils.py:33, :39, :44-48), reverse tour[min_i+1 .. min_j] of EVERY tour
+// (the reference applies each tour's own arg-min whenever the batch minimum passes the threshold), refresh dnext.
+__device__ __forceinline__ void twoopt_apply_batch(long long* __restrict__ tours, double* __restrict__ pos,
+                                                   double* __restrict__ dnext, const TwoOptCand* __restrict__ cand,
+                                                   TwoOptState* __restrict__ state, TwoOptCand* __restrict__ s_best,
+                                                   int N, int B, int ntiles, long long max_iterations) {
   if (state->done) return;
   __shared__ TwoOptCand s_red[32];
   // s_best: per-tour arg-min in global memory (any batch size; written by thread 0, read after __syncthreads)
@@ -402,4 +455,29 @@ __global__ void __launch_bounds__(1024) k_twoopt_apply(long long* __restrict__ t
     state->iterations = it;
     if (it >= max_iterations) state->done = 1;
   }
+}
+
+// Single block: one iteration of dfb_two_opt's batch.
+__global__ void __launch_bounds__(1024) k_twoopt_apply(long long* __restrict__ tours, double* __restrict__ pos,
+                                                       double* __restrict__ dnext, const TwoOptCand* __restrict__ cand,
+                                                       TwoOptState* __restrict__ state, TwoOptCand* __restrict__ s_best,
+                                                       int N, int B, int ntiles, long long max_iterations) {
+  twoopt_apply_batch(tours, pos, dnext, cand, state, s_best, N, B, ntiles, max_iterations);
+}
+
+// One block per instance: one iteration of its own batch, under its own stopping rule and cap.  An instance that stops
+// takes itself off *running, the counter the host polls.
+__global__ void __launch_bounds__(1024) k_twoopt_apply_instances(long long* __restrict__ tours, double* __restrict__ pos,
+                                                                 double* __restrict__ dnext,
+                                                                 const TwoOptCand* __restrict__ cand,
+                                                                 const TwoOptInst* __restrict__ insts,
+                                                                 TwoOptState* __restrict__ states,
+                                                                 TwoOptCand* __restrict__ s_best, int* __restrict__ running,
+                                                                 long long max_iterations) {
+  TwoOptState* st = states + blockIdx.x;
+  if (st->done) return;
+  const TwoOptInst in = insts[blockIdx.x];
+  twoopt_apply_batch(tours + in.tour0, pos + 2 * in.tour0, dnext + in.dnext0, cand + in.cand0, st, s_best + in.tour_first,
+                     in.n, in.B, in.ntiles, max_iterations);
+  if (threadIdx.x == 0 && st->done) atomicSub(running, 1);   // thread 0 is the one that sets done
 }

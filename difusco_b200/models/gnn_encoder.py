@@ -115,6 +115,7 @@ class GNNEncoder(nn.Module):
     self._weights_key = None
     self._graph_key = None
     self._points_key = None
+    self._n_segments = 0      # GroupNorm segments of the prepared graph: instances, dense samples or 1
     self._complete_cache = {}
 
   # ------------------------------------------------------------------------------------------
@@ -170,6 +171,7 @@ class GNNEncoder(nn.Module):
       else:
         ctx.prepare_graph_instances(ei.data_ptr(), int(num_nodes), int(ei.shape[1]), ptr, self._stream())
       self._graph_key = key
+      self._n_segments = int(gn_segments) if ptr is None else ptr.size - 1
       self._graph_hold = ei
       self._points_key = None
     return ctx

@@ -194,8 +194,12 @@ class COMetaModel(_Base):
                      torch.cuda.current_stream().cuda_stream)
     return (out, p) if want_prob else out
 
-  def _fused_loop(self, xt, steps, seed=None, record_steps=None):
+  def _fused_loop(self, xt, steps, seed=None, record_steps=None, instance_seeds=None):
     """The whole reverse-diffusion loop on device (pl_tsp_model.py:207-217).  In place on xt.
+
+    instance_seeds (a sequence of ints, one per instance of the prepared graph, or per sample of a dense call) keys
+    the sampling per instance instead of by the element's index in the call: each instance then draws what it draws
+    when denoised alone with seed=instance_seeds[i], whatever else is in the batch.
 
     record_steps (a list of step indices, or "all") also records those steps from inside the same loop and returns
     (xt, trace): trace["steps"] the recorded step indices, "t" their source timesteps t1, "xt" (n_rec, N) the state
@@ -212,17 +216,29 @@ class COMetaModel(_Base):
       t1s.append(int(t1))
       consts.append(c)
       lasts.append(last)
-    if seed is None:   # honour torch.manual_seed like the reference's torch.bernoulli would
+    seeds = None
+    if instance_seeds is not None:
+      if seed is not None:
+        raise ValueError("give seed or instance_seeds, not both")
+      seeds = _cabi.instance_seeds_array(instance_seeds, self.model._n_segments)
+    elif seed is None:   # honour torch.manual_seed like the reference's torch.bernoulli would
       seed = int(torch.randint(0, 2 ** 62, (1,)).item())
     mode = _cabi.CATEGORICAL if self.diffusion_type == "categorical" else _cabi.GAUSSIAN
     stream = torch.cuda.current_stream().cuda_stream
+    rec = []
+    if record_steps is not None:
+      rec = list(range(steps)) if isinstance(record_steps, str) and record_steps == "all" else \
+          [int(s) for s in record_steps]
+      if any(s < 0 or s >= steps for s in rec) or any(b <= a for a, b in zip(rec, rec[1:])):
+        raise ValueError(f"record_steps must be strictly increasing and inside [0, {steps}): {rec}")
+    d_seeds = None if seeds is None else torch.from_numpy(seeds.view(np.int64)).to(xt.device)
     if record_steps is None:
-      ctx.denoise(mode, xt.data_ptr(), t1s, consts, lasts, None, seed, stream)
+      if d_seeds is None:
+        ctx.denoise(mode, xt.data_ptr(), t1s, consts, lasts, None, seed, stream)
+      else:
+        ctx.denoise_instances(mode, xt.data_ptr(), t1s, consts, lasts, d_seeds.data_ptr(), seeds.size, (), None,
+                              None, None, stream)
       return xt
-    rec = list(range(steps)) if isinstance(record_steps, str) and record_steps == "all" else \
-        [int(s) for s in record_steps]
-    if any(s < 0 or s >= steps for s in rec) or any(b <= a for a, b in zip(rec, rec[1:])):
-      raise ValueError(f"record_steps must be strictly increasing and inside [0, {steps}): {rec}")
     n, dev = xt.numel(), xt.device
     out_channels = 2 if mode == _cabi.CATEGORICAL else 1
     trace = {"steps": torch.tensor(rec, dtype=torch.int64, device=dev),
@@ -231,6 +247,29 @@ class COMetaModel(_Base):
              "out": torch.empty((len(rec), n, out_channels), device=dev, dtype=torch.float32)}
     if mode == _cabi.CATEGORICAL:
       trace["p"] = torch.empty((len(rec), n), device=dev, dtype=torch.float32)
-    ctx.denoise_record(mode, xt.data_ptr(), t1s, consts, lasts, rec, trace["xt"].data_ptr(),
-                       trace["p"].data_ptr() if "p" in trace else None, trace["out"].data_ptr(), None, seed, stream)
+    ptrs = (trace["xt"].data_ptr(), trace["p"].data_ptr() if "p" in trace else None, trace["out"].data_ptr())
+    if d_seeds is None:
+      ctx.denoise_record(mode, xt.data_ptr(), t1s, consts, lasts, rec, *ptrs, None, seed, stream)
+    else:
+      ctx.denoise_instances(mode, xt.data_ptr(), t1s, consts, lasts, d_seeds.data_ptr(), seeds.size, rec, *ptrs,
+                            stream)
     return xt, trace
+
+  @staticmethod
+  def _solve_seeds(seeds, n):
+    """solve_batch's seeds -> n torch.Generators, instance i's seeded with seeds[i] alone."""
+    if isinstance(seeds, (str, bytes)) or not hasattr(seeds, "__len__"):
+      raise ValueError(f"seeds must be a sequence of integers, got {type(seeds).__name__}")
+    if len(seeds) != n:
+      raise ValueError(f"{len(seeds)} seeds for {n} instances")
+    gens = []
+    for s in seeds:
+      if isinstance(s, (bool, np.bool_)) or not isinstance(s, (int, np.integer)) or not 0 <= int(s) < 2 ** 63:
+        raise ValueError(f"seeds must be integers in [0, 2**63), got {s!r}")
+      gens.append(torch.Generator().manual_seed(int(s)))
+    return gens
+
+  @staticmethod
+  def _round_seed(gen):
+    """The Philox seed of one sequential round, drawn from the instance's own generator."""
+    return int(torch.randint(0, 2 ** 62, (1,), generator=gen).item())

@@ -6,6 +6,8 @@
   test_step(batch, batch_idx, draw=False, split='test')                   :142-209
 Greedy MIS decoding (mis_decode_np, :194-196; SURVEY 8f row f4) is `difusco_b200.utils.mis_utils.mis_decode_np`,
 applied by test_step exactly as the reference does (best of all samples -> `{split}/solved_cost`).
+solve_batch(batch, seeds, split='test') runs test_step for every graph of a collated batch at once, each graph's result
+independent of the rest of the batch.
 """
 import numpy as np
 import torch
@@ -32,17 +34,19 @@ class MISModel(COMetaModel):
   def gaussian_denoise_step(self, xt, t, device, edge_index=None, target_t=None):
     return self._denoise_step(xt, t, device, edge_index, target_t)
 
-  def denoise_labels(self, edge_index, xt, steps=None, seed=None, record_steps=None, node_ptr=None):
+  def denoise_labels(self, edge_index, xt, steps=None, seed=None, record_steps=None, node_ptr=None,
+                     instance_seeds=None):
     """xt0 (V,) -> raw final node labels on device, the whole loop fused.  record_steps (step indices or "all"):
     returns (labels, trace) instead, trace as COMetaModel._fused_loop: "xt" / "p" (n_rec, V), "out" (n_rec, V, out).
     node_ptr: node offsets of the graphs of a block-diagonal batch (PyG's Batch.ptr); each graph then gets its own
-    head GroupNorm, as if it were denoised alone."""
+    head GroupNorm, as if it were denoised alone.  instance_seeds (one int per graph of node_ptr, or one for the call):
+    sampling keyed per graph, so that each graph's labels are those it gets alone with that seed."""
     steps = steps or self.args.inference_diffusion_steps
     with torch.no_grad():
       dev = self.model._device()
       self.model.set_graph(edge_index.long().to(dev), xt.shape[0], 1, node_ptr)
       x = xt.reshape(-1).float().contiguous().to(dev).clone()
-      return self._fused_loop(x, steps, seed, record_steps)
+      return self._fused_loop(x, steps, seed, record_steps, instance_seeds)
 
   def test_step(self, batch, batch_idx, draw=False, split="test"):
     device = batch[-1].device
@@ -82,6 +86,61 @@ class MISModel(COMetaModel):
     self.last_predict_labels = predict_labels          # raw heatmaps of the last call (not part of the reference API)
     self.last_solved_cost = best_solved_cost
     return metrics
+
+  def solve_batch(self, batch, seeds, split="test"):
+    """test_step for every graph of a collated batch (index, graph, point_indicator): graph.x / graph.edge_index
+    concatenated in graph order with node offsets, point_indicator the node counts.  Each graph's parallel_sampling
+    replicas share one GroupNorm as in test_step; all graphs run in one fused loop per sequential round, then
+    mis_decode_np per graph.  seeds: one int per graph; its round seeds and initial noise come from a torch.Generator
+    seeded with seeds[i] alone and the sampling is keyed per graph, so its result does not depend on the other graphs.
+    Returns one metrics dict per graph with test_step's keys, and logs them as n test_step calls would."""
+    import scipy.sparse
+    _, graph_data, point_indicator = batch
+    labels = graph_data.x.reshape(-1)
+    edge_index = graph_data.edge_index.reshape(2, -1)
+    sizes = [int(c) for c in point_indicator.reshape(-1)]
+    if sum(sizes) != labels.shape[0] or min(sizes, default=0) < 1:
+      raise ValueError(f"point_indicator {sizes} does not match {labels.shape[0]} nodes")
+    gens = self._solve_seeds(seeds, len(sizes))
+    node0 = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+    ei = edge_index.cpu().numpy()
+    owner = np.searchsorted(node0, ei[0], side="right") - 1
+    if ei.size and (owner != np.searchsorted(node0, ei[1], side="right") - 1).any():
+      raise ValueError("an edge joins two graphs of the batch")
+    P, rounds = self.args.parallel_sampling, self.args.sequential_sampling
+    dev = self.model._device()
+    local = [np.ascontiguousarray(ei[:, owner == i] - node0[i]) for i in range(len(sizes))]
+    ptr = np.concatenate([[0], np.cumsum([P * n for n in sizes])]).astype(np.int64)
+    edges = torch.cat([self.duplicate_edge_index(torch.from_numpy(e).to(dev), n, dev) + int(ptr[i])
+                       for i, (e, n) in enumerate(zip(local, sizes))], 1)
+    samples = [[] for _ in sizes]
+    for _ in range(rounds):
+      round_seeds, noise = [], []
+      for g, n in zip(gens, sizes):
+        round_seeds.append(self._round_seed(g))
+        z = torch.randn(P * n, generator=g)
+        noise.append((z > 0).float() if self.diffusion_type != "gaussian" else z)
+      xt = self.denoise_labels(edges, torch.cat(noise), node_ptr=ptr, instance_seeds=round_seeds)
+      xt = xt.float().cpu().detach().numpy()
+      xt = xt * 0.5 + 0.5 if self.diffusion_type == "gaussian" else xt + 1e-6
+      for i, part in enumerate(np.split(xt, ptr[1:-1])):
+        samples[i].append(part)
+    out, costs = [], []
+    for i, n in enumerate(sizes):
+      adj_mat = scipy.sparse.coo_matrix((np.ones_like(local[i][0]), (local[i][0], local[i][1])))
+      predict_labels = np.concatenate(samples[i], axis=0)
+      solved = [mis_decode_np(pl, adj_mat) for pl in np.split(predict_labels, rounds * P)]
+      best = np.max([sol.sum() for sol in solved])
+      metrics = {f"{split}/gt_cost": labels[node0[i]:node0[i + 1]].cpu().numpy().sum()}
+      # batch_size=1: each value is one graph's, as test_step logs it; Lightning would otherwise weight it by the size
+      # it infers from the collated batch
+      for k, v in metrics.items():
+        self.log(k, v, on_epoch=True, sync_dist=True, batch_size=1)
+      self.log(f"{split}/solved_cost", best, prog_bar=True, on_epoch=True, sync_dist=True, batch_size=1)
+      out.append(metrics)
+      costs.append(best)
+    self.last_solved_costs = costs      # per-graph artefact of the last call (not part of the metrics)
+    return out
 
   def validation_step(self, batch, batch_idx):
     return self.test_step(batch, batch_idx, split="val")

@@ -5,6 +5,8 @@ Same method names and signatures on the denoise path:
   categorical_denoise_step(points, xt, t, device, edge_index=None, target_t=None)   :122-138
   gaussian_denoise_step(points, xt, t, device, edge_index=None, target_t=None)      :140-151
   test_step(batch, batch_idx, split='test')                                   :153-256
+plus solve_batch(batch, seeds, split='test'): test_step for the n instances of a collated batch in one fused loop per
+sequential round and one multi-instance 2-opt, each instance's result independent of the rest of the batch.
 test_step runs the reference's loop (:185-222) as ONE fused device loop, then the reference's decode
 (:227-256; SURVEY 8f rows f2/f3): merge_tours (host C++), batched 2-opt (CUDA), TSPEvaluator - and returns the
 reference's metrics dict.  `--save_numpy_heatmap` (:224-225, :258-267) is honoured.
@@ -15,7 +17,7 @@ import numpy as np
 import torch
 
 from .pl_meta_model import COMetaModel
-from .utils.tsp_utils import TSPEvaluator, batched_two_opt_torch, merge_tours
+from .utils.tsp_utils import TSPEvaluator, batched_two_opt_instances, batched_two_opt_torch, merge_tours
 
 
 def _shape_trace(trace, shape):
@@ -64,12 +66,16 @@ class TSPModel(COMetaModel):
     return self._denoise_step(points, xt, t, device, edge_index, target_t)
 
   # ------------------------------------------------------------------------------------
-  def denoise_heatmap(self, points, edge_index, xt, steps=None, seed=None, record_steps=None, node_ptr=None):
+  def denoise_heatmap(self, points, edge_index, xt, steps=None, seed=None, record_steps=None, node_ptr=None,
+                      instance_seeds=None):
     """xt0 -> raw final xt on device, the whole loop fused (no host sync inside).
 
     node_ptr (sparse only): node offsets of the instances of a block-diagonal batch (PyG's Batch.ptr); each instance
-    then gets its own head GroupNorm, as if it were denoised alone.  The sampling draws still depend on an edge's
-    position in the call.
+    then gets its own head GroupNorm, as if it were denoised alone.
+
+    instance_seeds (one int per instance of node_ptr, or per sample of a dense batch): sampling keyed per instance, so
+    that each instance's heat map is the one it gets alone with seed=instance_seeds[i], whatever else is in the call.
+    Without it the draws are keyed by an element's position in the call.
 
     record_steps (step indices or "all"): returns (heatmap, trace) instead, trace as COMetaModel._fused_loop with
     each tensor shaped like xt after its leading step dimension: (n_rec, E) sparse, (n_rec, B, V, V) dense; "out"
@@ -80,9 +86,9 @@ class TSPModel(COMetaModel):
       self._prepare(points.to(dev), edge_index.to(dev) if edge_index is not None else None, dev, node_ptr)
       x = xt.reshape(-1).float().contiguous().to(dev).clone()
       if record_steps is None:
-        self._fused_loop(x, steps, seed)
+        self._fused_loop(x, steps, seed, instance_seeds=instance_seeds)
         return x.reshape(xt.shape)
-      _, trace = self._fused_loop(x, steps, seed, record_steps)
+      _, trace = self._fused_loop(x, steps, seed, record_steps, instance_seeds)
       return x.reshape(xt.shape), _shape_trace(trace, xt.shape)
 
   # ------------------------------------------------------------------------------------
@@ -149,6 +155,114 @@ class TSPModel(COMetaModel):
     self.last_heatmap = heatmaps[0] if rounds == 1 else np.stack(heatmaps)
     self.last_solved_tours, self.last_solved_cost = refined, best
     return metrics
+
+  # ------------------------------------------------------------------------------------
+  # solve_batch: test_step for every instance of a collated batch at once
+  # ------------------------------------------------------------------------------------
+  def _instances(self, batch):
+    """n instances collated together -> per instance (points (n_i, 2) tensor, local edge_index (2, E_i) tensor or None,
+    ground-truth tour (n_i + 1,) numpy).  Sparse: TSPGraphDataset items collated by PyG (graph.x / graph.edge_index
+    concatenated in instance order with node offsets, point_indicator / edge_indicator the per-instance node and edge
+    counts, tours stacked (n, n_i + 1) or concatenated).  Dense: (index, points (B, N, 2), adj, tours (B, N + 1))."""
+    if not self.sparse:
+      _, coords, _, gt = batch
+      if coords.dim() != 3 or coords.shape[-1] != 2:
+        raise ValueError(f"dense points must be (B, N, 2), got {tuple(coords.shape)}")
+      gt = gt.reshape(coords.shape[0], -1).cpu().numpy()
+      return [(coords[i], None, gt[i]) for i in range(coords.shape[0])]
+    _, graph, point_indicator, edge_indicator, gt = batch
+    coords = graph.x.reshape((-1, 2))
+    edges = graph.edge_index.reshape((2, -1))
+    nodes = [int(c) for c in point_indicator.reshape(-1)]
+    counts = [int(c) for c in edge_indicator.reshape(-1)]
+    if len(nodes) != len(counts) or sum(nodes) != coords.shape[0] or sum(counts) != edges.shape[1]:
+      raise ValueError(f"point_indicator {nodes} / edge_indicator {counts} do not match {coords.shape[0]} nodes and "
+                       f"{edges.shape[1]} edges")
+    gt = gt.reshape(-1).cpu().numpy()
+    if gt.size != sum(nodes) + len(nodes):
+      raise ValueError(f"{gt.size} tour entries for instances of {nodes} nodes")
+    out, v0, e0 = [], 0, 0
+    for n, e in zip(nodes, counts):
+      ei = edges[:, e0:e0 + e] - v0
+      if e and (int(ei.min()) < 0 or int(ei.max()) >= n):
+        raise ValueError("each instance's edges must follow the previous instance's, inside its own nodes")
+      out.append((coords[v0:v0 + n], ei, gt[v0 + len(out):v0 + len(out) + n + 1]))
+      v0, e0 = v0 + n, e0 + e
+    return out
+
+  def solve_batch(self, batch, seeds, split="test"):
+    """test_step for every instance of a collated batch: each instance's parallel_sampling replicas in one fused
+    denoise loop per sequential round (the replicas of a sparse instance share one GroupNorm, as in test_step; a dense
+    replica is a sample of its own), then merge_tours per instance and round and one batched_two_opt_instances.
+
+    seeds: one int per instance.  Instance i's round seeds and initial noise come from a torch.Generator seeded with
+    seeds[i] alone and the sampling is keyed per instance, so its tours and metrics do not depend on the other
+    instances of the batch.  Returns one metrics dict per instance with test_step's keys, and logs them as n
+    test_step calls would."""
+    if getattr(self.args, "save_numpy_heatmap", False):
+      raise NotImplementedError("solve_batch does not save heat maps: use test_step for --save_numpy_heatmap")
+    inst = self._instances(batch)
+    gens = self._solve_seeds(seeds, len(inst))
+    copies, rounds = self.args.parallel_sampling, self.args.sequential_sampling
+    dev = self.model._device()
+    np_points = [p.cpu().numpy() for p, _, _ in inst]
+    if self.sparse:
+      sizes = [p.shape[0] for p in np_points]
+      ptr = np.concatenate([[0], np.cumsum([copies * n for n in sizes])]).astype(np.int64)
+      coords = torch.cat([p.repeat(copies, 1) for p, _, _ in inst])
+      edges = torch.cat([self.duplicate_edge_index(e.to(dev), n, dev) + int(ptr[i])
+                         for i, ((_, e, _), n) in enumerate(zip(inst, sizes))], 1)
+      lens = [copies * e.shape[1] for _, e, _ in inst]
+    else:
+      ptr = None
+      coords = torch.stack([p for p, _, _ in inst]).repeat_interleave(copies, 0)
+      edges = None
+      lens = [copies] * len(inst)
+    heats = []
+    for _ in range(rounds):
+      round_seeds, noise = [], []
+      for g, n_el in zip(gens, lens):
+        round_seeds += [self._round_seed(g) for _ in range(1 if self.sparse else copies)]
+        shape = (n_el,) if self.sparse else (copies,) + tuple(inst[0][0].shape[:1]) * 2
+        z = torch.randn(shape, generator=g)
+        noise.append((z > 0).float() if self.diffusion_type != "gaussian" else z)
+      xt = torch.cat(noise)
+      heat = self._heatmap_to_numpy(self.denoise_heatmap(coords, edges, xt, node_ptr=ptr, instance_seeds=round_seeds))
+      heats.append(np.split(heat, np.cumsum(lens)[:-1]))
+    exact = getattr(self.args, "exact_merge", True)
+    jobs = [(i, r) for i in range(len(inst)) for r in range(rounds)]
+
+    def merge(job):
+      i, r = job
+      e = inst[i][1]
+      return merge_tours(heats[r][i], np_points[i], None if e is None else e.cpu().numpy(), sparse_graph=self.sparse,
+                         parallel_sampling=copies, exact=exact)
+
+    from concurrent.futures import ThreadPoolExecutor
+    with ThreadPoolExecutor(max_workers=min(len(jobs), os.cpu_count() or 1)) as pool:
+      merged = list(pool.map(merge, jobs))
+    refined, iterations = batched_two_opt_instances(
+        [np_points[i].astype("float64") for i, _ in jobs], [np.array(t).astype("int64") for t, _ in merged],
+        max_iterations=getattr(self.args, "two_opt_iterations", 1000), device=dev)
+    out, tours_out, costs = [], [], []
+    for i in range(len(inst)):
+      k = [jobs.index((i, r)) for r in range(rounds)]
+      solved = np.concatenate([refined[j] for j in k], axis=0)
+      scorer = TSPEvaluator(np_points[i])
+      best = np.min([scorer.evaluate(solved[s]) for s in range(copies * rounds)])
+      metrics = {f"{split}/gt_cost": scorer.evaluate(inst[i][2]),
+                 f"{split}/2opt_iterations": iterations[k[-1]], f"{split}/merge_iterations": merged[k[-1]][1]}
+      # batch_size=1: each value is one instance's, as test_step logs it; Lightning would otherwise weight it by the
+      # size it infers from the collated batch
+      for name, value in metrics.items():
+        self.log(name, value, on_epoch=True, sync_dist=True, batch_size=1)
+      self.log(f"{split}/solved_cost", best, prog_bar=True, on_epoch=True, sync_dist=True, batch_size=1)
+      out.append(metrics)
+      tours_out.append(solved)
+      costs.append(best)
+    # not part of the metrics: per-instance artefacts of the last call
+    self.last_solved_tours, self.last_solved_costs = tours_out, costs
+    return out
 
   def run_save_numpy_heatmap(self, adj_mat, np_points, real_batch_idx, split):
     """--save_numpy_heatmap (pl_tsp_model.py:258-267): <save_dir>/<name>/<version>/numpy_heatmap/{split}-heatmap-<idx>.npy

@@ -3,6 +3,8 @@ denoise path in TSPModel.test_step (pl_tsp_model.py:227-247).
 
   merge_tours(adj_mat, np_points, edge_index_np, sparse_graph=False, parallel_sampling=1)   tsp_utils.py:89-145
   batched_two_opt_torch(points, tour, max_iterations=1000, device="cpu")                    tsp_utils.py:12-49
+  batched_two_opt_instances(points_list, tours_list, max_iterations=1000, device="cuda")   batched_two_opt_torch per
+                                                                                           instance, in one call
   TSPEvaluator(points).evaluate(route)                                                      tsp_utils.py:148-156
 
 merge_tours is host C++ in libdifusco_b200.so (csrc/tsp_decode.cuh): only the non-zero heat entries are sorted.  The
@@ -33,6 +35,14 @@ def batched_two_opt_torch(points, tour, max_iterations=1000, device="cuda"):
   """points (N, 2) float64 numpy, tour (B, N+1) int64 numpy -> (tour, iterations), both as the reference returns."""
   tours, iterations = _engine(device).two_opt(np.asarray(points, dtype=np.float64), tour, max_iterations)
   return tours, iterations
+
+
+def batched_two_opt_instances(points_list, tours_list, max_iterations=1000, device="cuda"):
+  """batched_two_opt_torch on many instances in one call: points_list[i] (n_i, 2), tours_list[i] (B_i, n_i + 1) of
+  local node ids -> (tours_list, iterations_list), each instance exactly as batched_two_opt_torch on it alone (its own
+  stopping rule and iteration cap)."""
+  _cabi.two_opt_instances_arrays(points_list, tours_list)   # argument checks before any device work
+  return _engine(device).two_opt_instances(points_list, tours_list, max_iterations)
 
 
 def _dense_order(points, heat, edge_index):

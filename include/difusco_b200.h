@@ -81,8 +81,8 @@ int dfb_prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_t num_nodes
  * GroupNorm: the reference's answer for every instance as if it were evaluated alone (its test loader's batch size 1,
  * pl_meta_model.py:194-198), at the throughput of one call.  node_ptr is a HOST array of n_instances + 1 elements in
  * PyG's Batch.ptr convention: instance i owns nodes [node_ptr[i], node_ptr[i+1]), and its GroupNorm runs over its
- * edges (TSP) or its nodes (MIS).  edge_index as for dfb_prepare_graph (need not be sorted).  Sampling is not per
- * instance: the Philox draws stay keyed by the element's index in the call.
+ * edges (TSP) or its nodes (MIS).  edge_index as for dfb_prepare_graph (need not be sorted).  dfb_denoise keys the
+ * Philox draws by the element's index in the call; dfb_denoise_instances keys them per instance.
  * DFB_E_INVALID, with the previously prepared graph left in use, when n_instances < 1, node_ptr[0] != 0,
  * node_ptr[n_instances] != num_nodes, node_ptr is not strictly increasing, an edge joins two instances, or a TSP
  * instance has no edges. */
@@ -110,7 +110,7 @@ int dfb_encoder_forward(dfb_ctx* ctx, const float* xt, float t, float* out, void
  *   last         1 when target_t == 0: categorical returns clamp(p, min=0) (the heatmap)
  *                instead of a Bernoulli sample (:139-142)
  *   uniforms     DEVICE (N,) injected U[0,1) (categorical) / N(0,1) (gaussian ddpm) draws or
- *                NULL -> in-kernel Philox4x32-10 keyed by (seed, step_index, element)
+ *                NULL -> in-kernel Philox4x32-10 keyed by (seed, step_index, element index in the call)
  *   xt_in/xt_out DEVICE (N,), N = E (TSP) or V (MIS); may alias
  *   p_out        DEVICE (N,) optional: pre-sampling probability p (categorical; gaussian leaves it untouched)
  *   net_out      DEVICE (N,out_channels) optional: raw network output */
@@ -143,6 +143,23 @@ int dfb_denoise_record(dfb_ctx* ctx, int diffusion_type, float* xt, int steps, c
                        const float* consts, const int32_t* last_flags, const float* uniforms, uint64_t seed,
                        int n_record, const int32_t* record_steps, float* rec_xt, float* rec_p, float* rec_out,
                        void* stream);
+
+/* dfb_denoise_record with sampling keyed per instance, so that each instance's draws, and with them its result, do
+ * not depend on the other instances of the call.  An instance is a GroupNorm segment of the prepared graph: an instance
+ * of dfb_prepare_graph_instances, or a sample of a dense call with gn_segments = B (one segment: the whole call).  The
+ * element (edge for TSP, node for MIS) of instance s is drawn with Philox4x32-10 keyed by
+ *   (instance_seeds[s], step, rank of the element among instance s's elements in the caller's element order)
+ * which is exactly the key dfb_denoise uses for it when the instance is denoised alone with seed instance_seeds[s]:
+ * its index in that call.
+ *   instance_seeds  DEVICE (n_instances,) uint64; n_instances must equal the prepared graph's segment count
+ * Everything else as dfb_denoise_record, without injected draws (dfb_denoise_record takes those).  The seeds travel in
+ * the per-step device table: this call and dfb_denoise replay the same captured graph for any seed set.  Bad arguments
+ * (a null or host seed pointer, a seed count that is not the segment count, and dfb_denoise_record's cases) return
+ * DFB_E_INVALID before any device work. */
+int dfb_denoise_instances(dfb_ctx* ctx, int diffusion_type, float* xt, int steps, const int32_t* t1,
+                          const float* consts, const int32_t* last_flags, const uint64_t* instance_seeds,
+                          int n_instances, int n_record, const int32_t* record_steps, float* rec_xt, float* rec_p,
+                          float* rec_out, void* stream);
 
 /* dfb_denoise replays the whole loop as ONE captured CUDA graph (on a stream of the library, fenced to `stream` by
  * events; re-captured only when the prepared graph, the buffers, the implementation switches or `steps` change).
@@ -187,6 +204,17 @@ int dfb_tsp_merge_order(int64_t n, const int64_t* order, int64_t count, int64_t*
 int dfb_two_opt(dfb_ctx* ctx, const double* points, int64_t n, int64_t* tours, int64_t batch, int64_t max_iterations,
                 int64_t* iterations_out, void* stream);
 
+/* dfb_two_opt over many instances in one call.  points (V,2) float64 HOST; instance i owns nodes
+ * [node_ptr[i], node_ptr[i+1]) and tours [tour_ptr[i], tour_ptr[i+1]) (both HOST, n_instances + 1 entries, starting at
+ * 0); tours HOST, the instances' rows of n_i + 1 LOCAL node ids concatenated, updated in place; iterations_out HOST
+ * (n_instances,).  Every instance's tours and iteration count are exactly dfb_two_opt's on that instance alone: the
+ * same moves and float64 arithmetic, its own batch-wide stopping rule and its own cap; an instance with a non-finite
+ * point on a tour is returned unchanged after 0 iterations while the others run.  n_i in [3, 46340], at least one
+ * tour per instance, no limit on the tour count of one instance; DFB_E_INVALID, tours untouched, otherwise. */
+int dfb_two_opt_instances(dfb_ctx* ctx, const double* points, const int64_t* node_ptr, int64_t n_instances,
+                          const int64_t* tour_ptr, int64_t* tours, int64_t max_iterations, int64_t* iterations_out,
+                          void* stream);
+
 /* Row f4: the MCTS solver's text heat map (tsp_mcts/convert_numpy_to_txt.py:57-73; parsed by tsp_mcts/code/TSP_IO.h:461-492):
  * "<n>\n" then n lines of n values "%.6f" separated by one blank.  matrix (n,n) float64 HOST.  HOST code, no context.
  * Returns DFB_E_INVALID when the file cannot be written. */
@@ -211,6 +239,11 @@ int dfb_debug_edge_gemm(dfb_ctx* ctx, int layer, const float* e_in, float* acc_o
  * aggregation: the time vector goes to e (TSP) or h (MIS); after the last TSP layer h is left unchanged, after the last
  * MIS layer e is.  Always reads e and h: never the categorical LUT, the MIS e0 = 0 or the cached layer-0 linears. */
 int dfb_debug_gnn_layer(dfb_ctx* ctx, int layer, float t, float* h, float* e, void* stream);
+
+/* Test hook: number of times this context has captured the dfb_denoise loop into a CUDA graph.  A call that replays
+ * the existing graph (same prepared graph, buffers, implementation switches and step count; any seed, seed set or
+ * record buffers) leaves it unchanged. */
+int64_t dfb_debug_loop_captures(const dfb_ctx* ctx);
 
 /* Tuning hook: per-phase cycle counters of the edge kernel; out must hold 32 unsigned 64-bit values (host).  Only the
  * timed product kernel records them (dfb_set_phase_timing); otherwise the values read back as zero.  Read-and-reset.

@@ -12,6 +12,7 @@ DFB_OK, DFB_E_INVALID, DFB_E_CUDA, DFB_E_UNSUPPORTED, DFB_E_NOMEM = 0, -1, -2, -
 CATEGORICAL, GAUSSIAN = 0, 1
 EDGE_IMPL_TC, EDGE_IMPL_FP32, EDGE_IMPL_TC1 = 0, 1, 2
 AGGREGATION = {"sum": 0, "mean": 1, "max": 2}
+HEAD_FORWARD, HEAD_CATEGORICAL, HEAD_GAUSSIAN = 0, 1, 2
 
 # every symbol include/difusco_b200.h declares (tests check the library exports all of them)
 SYMBOLS = [
@@ -20,7 +21,7 @@ SYMBOLS = [
     "dfb_encoder_forward", "dfb_denoise_step", "dfb_denoise", "dfb_denoise_record", "dfb_denoise_instances",
     "dfb_denoise_host",
     "dfb_launch_count", "dfb_profile_begin", "dfb_profile_end", "dfb_debug_edge_gemm", "dfb_debug_gnn_layer",
-    "dfb_debug_loop_captures",
+    "dfb_debug_head", "dfb_debug_entry", "dfb_debug_loop_captures",
     "dfb_debug_phase_cycles", "dfb_debug_watchdog", "dfb_knn_graph", "dfb_set_graph_capture",
     "dfb_set_phase_timing", "dfb_tsp_merge_sparse", "dfb_tsp_merge_order", "dfb_two_opt", "dfb_two_opt_instances",
     "dfb_write_heatmap_txt",
@@ -69,6 +70,8 @@ def lib():
   L.dfb_profile_end.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(i64)]
   L.dfb_debug_edge_gemm.argtypes = [vp, i32, vp, vp, vp]
   L.dfb_debug_gnn_layer.argtypes = [vp, i32, f32, vp, vp, vp]
+  L.dfb_debug_head.argtypes = [vp, i32, vp, C.POINTER(f32), i32, vp, u64, i32, vp, vp, vp, vp, vp, vp, vp]
+  L.dfb_debug_entry.argtypes = [vp, i32, vp, f32, vp, vp, vp, vp, vp, vp]
   L.dfb_debug_phase_cycles.argtypes = [vp, C.POINTER(C.c_uint64)]
   L.dfb_debug_watchdog.argtypes = [vp, C.POINTER(C.c_int)]
   L.dfb_set_graph_capture.argtypes = [vp, i32]
@@ -388,3 +391,19 @@ class Context(object):
     """Run GNN layer `layer` alone at timestep t, in place on device h (V,256) and e (E,256); e rows in the prepared
     graph's stable row-sorted order."""
     self._ck(lib().dfb_debug_gnn_layer(self._h, int(layer), float(t), h_ptr, e_ptr, stream))
+
+  def debug_head(self, mode, z_ptr, consts=(0, 0, 0, 0), last=0, uniforms_ptr=None, seed=0, step_index=0,
+                 instance_seeds_ptr=None, xt_in_ptr=None, xt_out_ptr=None, p_out_ptr=None, net_out_ptr=None,
+                 stats_out_ptr=None, stream=0):
+    """Run the head of a forward (mode HEAD_*) on device z (R,256): E row-sorted edges (TSP) or V nodes (MIS).  All
+    buffers are device pointers in the caller's order; stats_out (segments, 32, 2) gets the GroupNorm mean and rstd."""
+    c = (C.c_float * 4)(*[float(x) for x in consts])
+    self._ck(lib().dfb_debug_head(self._h, int(mode), z_ptr, c, int(last), uniforms_ptr,
+                                  int(seed) & 0xFFFFFFFFFFFFFFFF, int(step_index), instance_seeds_ptr, xt_in_ptr,
+                                  xt_out_ptr, p_out_ptr, net_out_ptr, stats_out_ptr, stream))
+
+  def debug_entry(self, diffusion, xt_ptr, t, h0_out_ptr=None, e0_out_ptr=None, tvec_out_ptr=None, h_out_ptr=None,
+                  e_out_ptr=None, stream=0):
+    """Run the forward up to and including layer 0 at timestep t on device xt; outputs as dfb_debug_entry documents."""
+    self._ck(lib().dfb_debug_entry(self._h, int(diffusion), xt_ptr, float(t), h0_out_ptr, e0_out_ptr, tvec_out_ptr,
+                                   h_out_ptr, e_out_ptr, stream))

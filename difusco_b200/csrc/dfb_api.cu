@@ -774,23 +774,23 @@ static int run_layer(dfb_ctx* ctx, int l, float* h, float* e, const float* uv0, 
   return DFB_OK;
 }
 
-// Forward + head (mode HEAD_*) of step i of the staged tables: time vectors tvec[i], posterior parameters and output
-// pointers d_steps[i].  xt is the network input and the posterior's state in, xt_out its state out.
-static int run_forward(dfb_ctx* ctx, int mode, int i, const float* xt, float* xt_out, const float* uniforms,
-                       cudaStream_t st) {
-  const float* tvec = (const float*)ctx->tvec.p + (size_t)i * ctx->L * H;
+// The part of a forward before layer 0 (gnn_encoder.py:394-396, :405-407): h = h0 of the points (TSP) or
+// node_embed(scalar_embed(xt)) (MIS) in the context's h, and layer 0's edge input: for categorical TSP *xt_lut = xt
+// (layer 0 reads the 2-row LUT), for Gaussian TSP e0 = edge_embed(scalar_embed(xt)) in the context's e (row-sorted),
+// for MIS *e_zero = 1 (e0 = 0).
+static int run_entry(dfb_ctx* ctx, int mode, const float* xt, const float** xt_lut, int* e_zero, cudaStream_t st) {
   const GraphDev& g = ctx->g;
   const int V = g.V, E = g.E;
   float* h = (float*)ctx->h.p;
   float* e = (float*)ctx->e.p;
-  const float* xt_lut = nullptr;
-  int e_zero = 0;
+  *xt_lut = nullptr;
+  *e_zero = 0;
   if (!ctx->node_only) {
     if (!ctx->points_ready) FAIL(ctx, DFB_E_INVALID, "dfb_set_points must be called before a TSP forward");
     CK(ctx, cudaMemcpyAsync(h, ctx->h0.p, (size_t)V * H * sizeof(float), cudaMemcpyDeviceToDevice, st));
     if (mode == HEAD_CATEGORICAL) {   // the state is in {0,1}
-      xt_lut = xt;   // layer 0 reads the 2-row LUT instead of a materialised e0
-    } else {         // general values (Gaussian diffusion): e0 = edge_embed(edge_pos_embed(xt))
+      *xt_lut = xt;   // layer 0 reads the 2-row LUT instead of a materialised e0
+    } else {          // general values (Gaussian diffusion): e0 = edge_embed(edge_pos_embed(xt))
       const int CH = 65536;
       for (int s0 = 0; s0 < E; s0 += CH) {
         int n = std::min(CH, E - s0);
@@ -811,27 +811,52 @@ static int run_forward(dfb_ctx* ctx, int mode, int i, const float* xt, float* xt
       int r = embed_rows(ctx, 1, (const float*)ctx->feat.p, h + (size_t)v0 * H, n, st);
       if (r) return r;
     }
-    e_zero = 1;   // gnn_encoder.py:407: e0 = zeros
+    *e_zero = 1;   // gnn_encoder.py:407: e0 = zeros
   }
-  for (int l = 0; l < ctx->L; ++l) {
-    const bool first = l == 0;
-    int r = run_layer(ctx, l, h, e, (first && !ctx->node_only) ? (const float*)ctx->uvab0.p : nullptr,
-                      tvec + (size_t)l * H, first ? e_zero : 0, first ? xt_lut : nullptr, st);
-    if (r) return r;
-  }
-  // head
-  const float* Z = ctx->node_only ? h : e;
-  const int R = ctx->node_only ? V : E;
+  return DFB_OK;
+}
+
+// Layer l of a forward at time vectors tvec [L][256]: layer 0 takes run_entry's step-invariant inputs.
+static int run_forward_layer(dfb_ctx* ctx, int l, const float* tvec, const float* xt_lut, int e_zero, cudaStream_t st) {
+  const bool first = l == 0;
+  return run_layer(ctx, l, (float*)ctx->h.p, (float*)ctx->e.p,
+                   (first && !ctx->node_only) ? (const float*)ctx->uvab0.p : nullptr, tvec + (size_t)l * H,
+                   first ? e_zero : 0, first ? xt_lut : nullptr, st);
+}
+
+// The head of a forward (gnn_encoder.py:400-401, :412-413) on Z, the prepared graph's head rows (E row-sorted edges for
+// TSP, V nodes for MIS): GroupNorm statistics of each segment into gn_stats, then k_head with its posterior (mode
+// HEAD_*) and the outputs of the device step row sp, in the caller's order.
+static int run_head(dfb_ctx* ctx, int mode, const StepParams* sp, const float* Z, const float* xt, float* xt_out,
+                    const float* uniforms, cudaStream_t st) {
+  const int R = ctx->node_only ? ctx->g.V : ctx->g.E;
   k_gn_partial<<<ctx->gn_blocks, 256, 0, st>>>(Z, ctx->gseg, (double*)ctx->gn_part.p);
   CKL(ctx);
-  k_gn_final<<<dim3(ctx->gseg.n_segs, 32), 256, 0, st>>>((const double*)ctx->gn_part.p, Z, ctx->gseg,
+  k_gn_final<<<dim3(ctx->gseg.n_segs, 32), 256, 0, st>>>((const double*)ctx->gn_part.p, ctx->gseg,
                                                          (float*)ctx->gn_stats.p);
   CKL(ctx);
-  const PosteriorArgs pa{mode, ctx->d_steps + i, xt, xt_out, uniforms};
+  const PosteriorArgs pa{mode, sp, xt, xt_out, uniforms};
   k_head<<<(R + HEAD_THREADS - 1) / HEAD_THREADS, HEAD_THREADS, 0, st>>>(Z, R, ctx->gseg, (const float*)ctx->gn_stats.p,
-                                      ctx->node_only ? nullptr : g.perm, ctx->hp, pa);
+                                      ctx->node_only ? nullptr : ctx->g.perm, ctx->hp, pa);
   CKL(ctx);
   return DFB_OK;
+}
+
+// Forward + head (mode HEAD_*) of step i of the staged tables: time vectors tvec[i], posterior parameters and output
+// pointers d_steps[i].  xt is the network input and the posterior's state in, xt_out its state out.
+static int run_forward(dfb_ctx* ctx, int mode, int i, const float* xt, float* xt_out, const float* uniforms,
+                       cudaStream_t st) {
+  const float* tvec = (const float*)ctx->tvec.p + (size_t)i * ctx->L * H;
+  const float* xt_lut;
+  int e_zero;
+  int r = run_entry(ctx, mode, xt, &xt_lut, &e_zero, st);
+  if (r) return r;
+  for (int l = 0; l < ctx->L; ++l) {
+    r = run_forward_layer(ctx, l, tvec, xt_lut, e_zero, st);
+    if (r) return r;
+  }
+  return run_head(ctx, mode, ctx->d_steps + i, ctx->node_only ? (const float*)ctx->h.p : (const float*)ctx->e.p, xt,
+                  xt_out, uniforms, st);
 }
 
 // One staging path for every call that runs the time MLP: stage_acquire hands out a pinned slot, the caller fills
@@ -1155,6 +1180,94 @@ extern "C" int dfb_debug_gnn_layer(dfb_ctx* ctx, int layer, float t, float* h, f
   r = stage_commit(ctx, slot, 1, st);
   if (r) return r;
   return run_layer(ctx, layer, h, e, nullptr, (const float*)ctx->tvec.p + (size_t)layer * H, 0, nullptr, st);
+}
+
+// Test hook: the head of a forward (run_head) on the caller's z, with one step row staged as dfb_denoise_step stages it.
+extern "C" int dfb_debug_head(dfb_ctx* ctx, int mode, const float* z, const float* consts, int last,
+                              const float* uniforms, uint64_t seed, int step_index, const uint64_t* instance_seeds,
+                              const float* xt_in, float* xt_out, float* p_out, float* net_out, float* stats_out,
+                              void* stream_) {
+  if (!ctx) return DFB_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream_;
+  CK(ctx, cudaSetDevice(ctx->device));
+  if (!ctx->graph_ready) FAIL(ctx, DFB_E_INVALID, "dfb_prepare_graph must be called first");
+  int hm = HEAD_FORWARD;
+  if (mode == DFB_HEAD_CATEGORICAL || mode == DFB_HEAD_GAUSSIAN) {
+    int r = head_mode(ctx, mode == DFB_HEAD_CATEGORICAL ? DFB_DIFFUSION_CATEGORICAL : DFB_DIFFUSION_GAUSSIAN, &hm);
+    if (r) return r;
+    if (!xt_in || !xt_out) FAIL(ctx, DFB_E_INVALID, "a posterior mode needs xt_in and xt_out");
+  } else if (mode != DFB_HEAD_FORWARD) {
+    FAIL(ctx, DFB_E_INVALID, "unknown head mode %d", mode);
+  }
+  if (p_out && hm != HEAD_CATEGORICAL) FAIL(ctx, DFB_E_INVALID, "p_out is the categorical posterior's");
+  if (instance_seeds && uniforms) FAIL(ctx, DFB_E_INVALID, "instance_seeds key the Philox draws: no uniforms with them");
+  const void* dev[] = {z, uniforms, instance_seeds, xt_in, xt_out, p_out, net_out, stats_out};
+  for (const void* p : dev)
+    if (p && !is_device_ptr(p)) FAIL(ctx, DFB_E_INVALID, "z and every buffer must be device pointers");
+  if (!z) FAIL(ctx, DFB_E_INVALID, "z is required");
+  int slot;
+  int r = stage_acquire(ctx, &slot);
+  if (r) return r;
+  ctx->h_tvals[slot][0] = 0.0f;
+  StepParams& sp = ctx->h_steps[slot][0];
+  sp = StepParams{};
+  if (consts)
+    for (int k = 0; k < 4; ++k) sp.c[k] = consts[k];
+  sp.last = last;
+  sp.step = (unsigned)step_index;
+  sp.seed = seed;
+  sp.inst_seeds = (const unsigned long long*)instance_seeds;
+  sp.rec_out = net_out;
+  sp.rec_p = p_out;
+  r = stage_commit(ctx, slot, 1, st);
+  if (r) return r;
+  r = run_head(ctx, hm, ctx->d_steps, z, xt_in, xt_out, uniforms, st);
+  if (r) return r;
+  if (stats_out)
+    CK(ctx, cudaMemcpyAsync(stats_out, ctx->gn_stats.p, (size_t)ctx->gseg.n_segs * 32 * 2 * sizeof(float),
+                            cudaMemcpyDeviceToDevice, st));
+  return DFB_OK;
+}
+
+// Test hook: the part of a forward before layer 0 (run_entry) and layer 0 as the forward runs it, at timestep t.
+extern "C" int dfb_debug_entry(dfb_ctx* ctx, int diffusion_type, const float* xt, float t, float* h0_out, float* e0_out,
+                               float* tvec_out, float* h_out, float* e_out, void* stream_) {
+  if (!ctx) return DFB_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream_;
+  CK(ctx, cudaSetDevice(ctx->device));
+  if (!ctx->graph_ready) FAIL(ctx, DFB_E_INVALID, "dfb_prepare_graph must be called first");
+  int mode;
+  int r = head_mode(ctx, diffusion_type, &mode);
+  if (r) return r;
+  const void* dev[] = {xt, h0_out, e0_out, tvec_out, h_out, e_out};
+  for (const void* p : dev)
+    if (p && !is_device_ptr(p)) FAIL(ctx, DFB_E_INVALID, "xt and every output must be device pointers");
+  if (!xt) FAIL(ctx, DFB_E_INVALID, "xt is required");
+  int slot;
+  r = stage_acquire(ctx, &slot);
+  if (r) return r;
+  ctx->h_tvals[slot][0] = t;
+  ctx->h_steps[slot][0] = StepParams{};
+  r = stage_commit(ctx, slot, 1, st);
+  if (r) return r;
+  const float* xt_lut;
+  int e_zero;
+  r = run_entry(ctx, mode, xt, &xt_lut, &e_zero, st);
+  if (r) return r;
+  const size_t V = ctx->g.V, E = ctx->g.E, row = H * sizeof(float);
+  if (h0_out) CK(ctx, cudaMemcpyAsync(h0_out, ctx->h.p, V * row, cudaMemcpyDeviceToDevice, st));
+  if (e0_out && xt_lut) {   // the rows layer 0 reads from the LUT, as the fp32 edge layer materialises them
+    k_lut_expand<<<(ctx->g.E + 3) / 4, 256, 0, st>>>(xt_lut, ctx->g.perm, ctx->lut, e0_out, ctx->g.E);
+    CKL(ctx);
+  } else if (e0_out && !e_zero) {
+    CK(ctx, cudaMemcpyAsync(e0_out, ctx->e.p, E * row, cudaMemcpyDeviceToDevice, st));
+  }
+  if (tvec_out) CK(ctx, cudaMemcpyAsync(tvec_out, ctx->tvec.p, ctx->L * row, cudaMemcpyDeviceToDevice, st));
+  r = run_forward_layer(ctx, 0, (const float*)ctx->tvec.p, xt_lut, e_zero, st);
+  if (r) return r;
+  if (h_out) CK(ctx, cudaMemcpyAsync(h_out, ctx->h.p, V * row, cudaMemcpyDeviceToDevice, st));
+  if (e_out) CK(ctx, cudaMemcpyAsync(e_out, ctx->e.p, E * row, cudaMemcpyDeviceToDevice, st));
+  return DFB_OK;
 }
 
 // Test/tuning hook: read and reset the per-phase cycle counters of the edge kernel (slots PH_* of edge_layer_tc.cuh).

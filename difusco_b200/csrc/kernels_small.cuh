@@ -197,10 +197,13 @@ __global__ void __launch_bounds__(256) k_node_update(float* __restrict__ h, cons
 // batch dim is 1, so every edge of the call shares the statistics; nn.py:17-19).
 // A segment is a run of consecutive head rows normalised on its own: one per call, one per dense sample, or one per
 // instance of a ragged batch (dfb_prepare_graph_instances).  GnSegments holds the table dfb_prepare_graph builds.
-// fp32 runs of <= 32 rows, combined in fp64 partials: 3.2 M values per group would lose the 1e-4 contract in fp32
-// E[x^2]-E[x]^2 form (the reference's own CPU channels-last kernel does lose it when |mean|>>std).  The runs sum
-// x - pivot, with one pivot per (segment, group): the group's first channel in the segment's first row.  Without it
-// the fp32 runs of x^2 round at |mean|^2 * 2^-24, which is the whole variance once |mean| / std reaches ~1000.
+// Each thread (channel) takes fp32 runs of <= 32 rows held in registers, two passes each: the run's fp32 mean m, then
+// the sums of d = x - m and d^2.  A run's (count, mean, M2) goes to fp64 and the runs, the 8 channels of a group, the
+// blocks and the warps are merged with Chan's pairwise update.  So every fp32 sum is centred on its own run: its
+// rounding is relative to the run's own spread, and no single row (an outlier, a segment's structurally special first
+// row) and no offset |mean| / std sets the error.  A one-pass E[x^2] - E[x]^2 form rounds at |mean|^2 * 2^-24, the
+// whole variance once |mean| / std reaches ~1000 (the reference's own CPU channels-last kernel loses the 1e-4
+// contract there); a shift by one fixed row per segment instead cancels (distance of that row from the mean)^2.
 // ---------------------------------------------------------------------------------------------
 constexpr int GN_ROWS_PER_BLOCK = 256;
 struct GnSegments {
@@ -213,68 +216,82 @@ struct GnSegments {
   // there is more than one segment; otherwise that rank is the caller index minus the segment's first row.
   const int* local;
 };
-__device__ __forceinline__ float gn_pivot(const float* Z, int seg_row0, int group) {
-  return Z[(size_t)seg_row0 * H + group * 8];
+// (n, mean, M2) of a set of values += the disjoint set (nb, mb, m2b): Chan, Golub and LeVeque's pairwise update.  An
+// empty set is (0, 0, 0) on either side.
+__device__ __forceinline__ void chan_merge(double& n, double& mean, double& m2, double nb, double mb, double m2b) {
+  if (nb == 0.0) return;
+  const double nn = n + nb, d = mb - mean, f = nb / nn;
+  mean += d * f;
+  m2 += m2b + d * d * n * f;
+  n = nn;
+}
+// chan_merge with the set held by lane ^ off
+__device__ __forceinline__ void chan_merge_xor(double& n, double& mean, double& m2, int off) {
+  const double nb = __shfl_xor_sync(0xffffffffu, n, off), mb = __shfl_xor_sync(0xffffffffu, mean, off),
+               m2b = __shfl_xor_sync(0xffffffffu, m2, off);
+  chan_merge(n, mean, m2, nb, mb, m2b);
 }
 __global__ void __launch_bounds__(256) k_gn_partial(const float* __restrict__ Z, GnSegments sg,
-                                                    double* __restrict__ part) {
-  // one block per entry of sg.blk.  thread = channel; fp32 run of <= 32 rows, then fp64.
+                                                    double* __restrict__ part /* [blocks][32][2] mean, M2 */) {
+  // one block per entry of sg.blk.  thread = channel; fp32 runs of <= 32 rows in registers, then fp64.
   const int c = threadIdx.x;
   const int2 bk = sg.blk[blockIdx.x];
   const int r0 = bk.y;
   const int r1 = min(r0 + GN_ROWS_PER_BLOCK, sg.start[bk.x + 1]);
   const float* base = Z + c;
-  const float piv = gn_pivot(Z, sg.start[bk.x], c >> 3);
-  double S = 0.0, Q = 0.0;
+  double n = 0.0, mean = 0.0, m2 = 0.0;
   for (int r = r0; r < r1; r += 32) {
-    float s = 0.f, q = 0.f;
-    int re = min(r + 32, r1);
-    for (int rr = r; rr < re; ++rr) {
-      float v = base[(size_t)rr * H] - piv;
-      s += v;
-      q = fmaf(v, v, q);
-    }
-    S += (double)s;
-    Q += (double)q;
-  }
-  // reduce the 8 channels of a group (adjacent lanes)
+    const int m = min(32, r1 - r);
+    float v[32], s = 0.f;
 #pragma unroll
-  for (int o = 4; o > 0; o >>= 1) {
-    S += __shfl_xor_sync(0xffffffffu, S, o);
-    Q += __shfl_xor_sync(0xffffffffu, Q, o);
+    for (int i = 0; i < 32; ++i) {
+      v[i] = (i < m) ? base[(size_t)(r + i) * H] : 0.0f;
+      s += v[i];
+    }
+    const float mr = s / (float)m;
+    float s1 = 0.f, q = 0.f;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const float d = (i < m) ? v[i] - mr : 0.0f;
+      s1 += d;
+      q = fmaf(d, d, q);
+    }
+    const double dm = (double)s1 / m;   // the run's mean - mr
+    chan_merge(n, mean, m2, (double)m, (double)mr + dm, (double)q - (double)s1 * dm);
   }
+  // the 8 channels of a group (adjacent lanes)
+#pragma unroll
+  for (int o = 1; o < 8; o <<= 1) chan_merge_xor(n, mean, m2, o);
   if ((c & 7) == 0) {
     size_t o = ((size_t)blockIdx.x * 32 + (c >> 3)) * 2;
-    part[o] = S;
-    part[o + 1] = Q;
+    part[o] = mean;
+    part[o + 1] = m2;
   }
 }
-__global__ void __launch_bounds__(256) k_gn_final(const double* __restrict__ part, const float* __restrict__ Z,
-                                                  GnSegments sg, float* __restrict__ stats /* [segs][32][2] mean, rstd */) {
+__global__ void __launch_bounds__(256) k_gn_final(const double* __restrict__ part, GnSegments sg,
+                                                  float* __restrict__ stats /* [segs][32][2] mean, rstd */) {
   // grid (segs, 32 groups); 256 threads stride over the segment's block partials, then a fixed-shape fp64 tree
   // (warp shuffles + 8 warp results in shared memory): deterministic
-  __shared__ double sh[8][2];
+  __shared__ double sh[8][3];
   const int seg = blockIdx.x, gidx = blockIdx.y, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int b0 = sg.blk_first[seg], nb = sg.blk_first[seg + 1] - b0;
-  double S = 0.0, Q = 0.0;
+  const int s0 = sg.start[seg], s1 = sg.start[seg + 1];
+  double n = 0.0, mean = 0.0, m2 = 0.0;
   for (int b = threadIdx.x; b < nb; b += 256) {
-    size_t o = (((size_t)b0 + b) * 32 + gidx) * 2;
-    S += part[o];
-    Q += part[o + 1];
+    const size_t o = (((size_t)b0 + b) * 32 + gidx) * 2;
+    const int rb = s0 + b * GN_ROWS_PER_BLOCK;   // block b of the segment starts at this row (dfb_prepare_graph)
+    chan_merge(n, mean, m2, 8.0 * (min(rb + GN_ROWS_PER_BLOCK, s1) - rb), part[o], part[o + 1]);
   }
-  S = warp_sum_d(S);
-  Q = warp_sum_d(Q);
-  if (lane == 0) { sh[w][0] = S; sh[w][1] = Q; }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) chan_merge_xor(n, mean, m2, o);
+  if (lane == 0) { sh[w][0] = n; sh[w][1] = mean; sh[w][2] = m2; }
   __syncthreads();
   if (threadIdx.x == 0) {
-    S = 0.0; Q = 0.0;
-    for (int i = 0; i < 8; ++i) { S += sh[i][0]; Q += sh[i][1]; }
-    const int s0 = sg.start[seg];
-    double n = (double)(sg.start[seg + 1] - s0) * 8.0;
-    double dm = S / n;                       // mean - pivot
-    double var = Q / n - dm * dm;
+    n = sh[0][0]; mean = sh[0][1]; m2 = sh[0][2];
+    for (int i = 1; i < 8; ++i) chan_merge(n, mean, m2, sh[i][0], sh[i][1], sh[i][2]);
+    double var = m2 / n;
     if (var < 0.0) var = 0.0;
-    stats[((size_t)seg * 32 + gidx) * 2] = (float)((double)gn_pivot(Z, s0, gidx) + dm);
+    stats[((size_t)seg * 32 + gidx) * 2] = (float)mean;
     stats[((size_t)seg * 32 + gidx) * 2 + 1] = (float)(1.0 / sqrt(var + (double)LN_EPS));
   }
 }

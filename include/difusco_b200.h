@@ -39,6 +39,8 @@ enum { DFB_TASK_TSP = 0, DFB_TASK_MIS = 1 };               /* pl_tsp_model.py / 
 enum { DFB_DIFFUSION_CATEGORICAL = 0, DFB_DIFFUSION_GAUSSIAN = 1 }; /* pl_meta_model.py:27-36           */
 enum { DFB_EDGE_IMPL_TC = 0, DFB_EDGE_IMPL_FP32 = 1, DFB_EDGE_IMPL_TC1 = 2 }; /* wgmma product path (128-row tiles, two
   consumer warpgroups) / fp32 validation kernel / the wgmma kernel with 64-row tiles, one warpgroup (A/B and validation) */
+/* What dfb_debug_head runs after the network output: nothing, the categorical or the Gaussian posterior. */
+enum { DFB_HEAD_FORWARD = 0, DFB_HEAD_CATEGORICAL = 1, DFB_HEAD_GAUSSIAN = 2 };
 
 typedef struct dfb_ctx dfb_ctx;
 
@@ -239,6 +241,29 @@ int dfb_debug_edge_gemm(dfb_ctx* ctx, int layer, const float* e_in, float* acc_o
  * aggregation: the time vector goes to e (TSP) or h (MIS); after the last TSP layer h is left unchanged, after the last
  * MIS layer e is.  Always reads e and h: never the categorical LUT, the MIS e0 = 0 or the cached layer-0 linears. */
 int dfb_debug_gnn_layer(dfb_ctx* ctx, int layer, float t, float* h, float* e, void* stream);
+
+/* Test hook: the head of a forward alone (GroupNorm statistics of each segment of the prepared graph, GroupNorm, ReLU,
+ * 1x1 conv, then the posterior of `mode`, DFB_HEAD_*) on a DEVICE z (R,256) fp32: R = E rows in the prepared graph's
+ * row-sorted order for TSP, V rows in node order for MIS.  The segment table, perm and per-instance rank table of the
+ * prepared graph and the loaded head weights are used as a forward uses them; the step's row (consts, last, seed,
+ * step_index, instance_seeds) is staged as dfb_denoise_step stages it.  uniforms (R,) replace the Philox draws;
+ * instance_seeds (one uint64 per segment, DEVICE) key them per instance as dfb_denoise_instances does.  xt_in / xt_out
+ * (R,) are required by the posterior modes; p_out (R,) is categorical only; net_out (R, out_channels); stats_out
+ * (segments, 32, 2) receives each segment's GroupNorm mean and rstd.  Every buffer is DEVICE memory and in the caller's
+ * order; any output may be null.  Returns DFB_E_INVALID, writing nothing, on a bad mode, a mode the head's out_channels
+ * does not fit, or a host pointer. */
+int dfb_debug_head(dfb_ctx* ctx, int mode, const float* z, const float* consts, int last, const float* uniforms,
+                   uint64_t seed, int step_index, const uint64_t* instance_seeds, const float* xt_in, float* xt_out,
+                   float* p_out, float* net_out, float* stats_out, void* stream);
+
+/* Test hook: the part of a forward before layer 0, and layer 0 as the forward runs it, at timestep t on the DEVICE
+ * state xt (E,) for TSP or (V,) for MIS in the caller's order.  Categorical TSP reads the 2-row edge-embedding LUT,
+ * Gaussian TSP embeds xt, MIS starts from e0 = 0; TSP uses h0 and the cached layer-0 node linears of dfb_set_points.
+ * Optional DEVICE outputs: h0_out (V,256) the node embedding; e0_out (E,256, row-sorted) the edge embedding layer 0
+ * reads (for categorical TSP the LUT rows xt selects; for MIS untouched); tvec_out (n_layers,256) the time vectors of
+ * t; h_out (V,256) and e_out (E,256, row-sorted) after layer 0. */
+int dfb_debug_entry(dfb_ctx* ctx, int diffusion_type, const float* xt, float t, float* h0_out, float* e0_out,
+                    float* tvec_out, float* h_out, float* e_out, void* stream);
 
 /* Test hook: number of times this context has captured the dfb_denoise loop into a CUDA graph.  A call that replays
  * the existing graph (same prepared graph, buffers, implementation switches and step count; any seed, seed set or

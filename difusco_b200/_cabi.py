@@ -18,7 +18,7 @@ HEAD_FORWARD, HEAD_CATEGORICAL, HEAD_GAUSSIAN = 0, 1, 2
 SYMBOLS = [
     "dfb_abi_version", "dfb_create", "dfb_destroy", "dfb_last_error", "dfb_set_aggregation",
     "dfb_set_edge_impl", "dfb_load_weights", "dfb_prepare_graph", "dfb_prepare_graph_instances", "dfb_set_points",
-    "dfb_encoder_forward", "dfb_denoise_step", "dfb_denoise", "dfb_denoise_record", "dfb_denoise_instances",
+    "dfb_encoder_forward", "dfb_encoder_forward_timesteps", "dfb_denoise_step", "dfb_denoise", "dfb_denoise_record", "dfb_denoise_instances",
     "dfb_denoise_host",
     "dfb_launch_count", "dfb_profile_begin", "dfb_profile_end", "dfb_debug_edge_gemm", "dfb_debug_gnn_layer",
     "dfb_debug_head", "dfb_debug_entry", "dfb_debug_loop_captures",
@@ -53,6 +53,7 @@ def lib():
   L.dfb_prepare_graph_instances.argtypes = [vp, vp, i64, i64, i32, C.POINTER(i64), vp]
   L.dfb_set_points.argtypes = [vp, vp, vp]
   L.dfb_encoder_forward.argtypes = [vp, vp, f32, vp, vp]
+  L.dfb_encoder_forward_timesteps.argtypes = [vp, vp, i32, C.POINTER(f32), vp, vp, vp]
   L.dfb_denoise_step.argtypes = [vp, i32, vp, f32, C.POINTER(f32), i32, vp, u64, i32, vp, vp, vp, vp]
   L.dfb_denoise.argtypes = [vp, i32, vp, i32, C.POINTER(C.c_int32), C.POINTER(f32),
                             C.POINTER(C.c_int32), vp, u64, vp]
@@ -270,6 +271,13 @@ class Context(object):
   # ---- compute ----
   def encoder_forward(self, xt_ptr, t, out_ptr, stream=0):
     self._ck(lib().dfb_encoder_forward(self._h, xt_ptr, float(t), out_ptr, stream))
+
+  def encoder_forward_timesteps(self, xt_ptr, t_values, t_index_ptr, out_ptr, stream=0):
+    """encoder_forward with a timestep per element: t_values the distinct timesteps (host sequence), t_index_ptr a
+    device int32 (N,) array of positions in t_values, or None for every element at t_values[0]."""
+    v = np.ascontiguousarray(t_values, dtype=np.float32).reshape(-1)
+    self._ck(lib().dfb_encoder_forward_timesteps(self._h, xt_ptr, v.size, v.ctypes.data_as(C.POINTER(C.c_float)),
+                                                 t_index_ptr, out_ptr, stream))
 
   def denoise_step(self, diffusion, xt_in_ptr, t, consts, last, uniforms_ptr, seed, step_index, xt_out_ptr,
                    p_out_ptr=None, net_out_ptr=None, stream=0):

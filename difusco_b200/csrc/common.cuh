@@ -78,4 +78,18 @@ struct GraphDev {
   int n_pairs;
 };
 
+// A timestep per element (dfb_encoder_forward_timesteps).  The time vectors of the call's n distinct timesteps lie
+// `stride` floats apart (tvec [n][L][256]: stride L * 256), and element i, in the caller's order, adds the row of
+// timestep index[i].  An index outside [0, n) selects row n, which holds NaN, instead of reading out of bounds.
+struct TimeRows {
+  const int* index;   // [N] (E edges for TSP, V nodes for MIS); nullptr: one timestep for the whole call
+  int n;
+  int stride;
+};
+// layer vector tv (row 0 of the layer) -> the row of caller element i
+__device__ __forceinline__ const float* time_row(const float* tv, const TimeRows& tr, int i) {
+  const unsigned k = (unsigned)__ldg(tr.index + i);
+  return tv + (size_t)(k < (unsigned)tr.n ? k : (unsigned)tr.n) * tr.stride;
+}
+
 }  // namespace dfb

@@ -710,8 +710,8 @@ extern "C" int dfb_set_points(dfb_ctx* ctx, const float* points, void* stream_) 
 // ================================================================================================
 // one forward (+ optional fused posterior)
 // ================================================================================================
-static int launch_edge_layer(dfb_ctx* ctx, int l, float* e, const float* uvab, const float* tvec_edge, int write_e,
-                             int e_zero, const float* xt_for_lut, cudaStream_t st) {
+static int launch_edge_layer(dfb_ctx* ctx, int l, float* e, const float* uvab, const float* tvec_edge,
+                             const TimeRows& tr, int write_e, int e_zero, const float* xt_for_lut, cudaStream_t st) {
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   if (ctx->profiling) {
     if (ctx->ev_used + 2 > ctx->ev_pool.size()) {
@@ -733,12 +733,12 @@ static int launch_edge_layer(dfb_ctx* ctx, int l, float* e, const float* uvab, c
       CKL(ctx);
     }
     k_edge_layer_fp32<<<ctx->g.n_groups, 256, EF_SMEM, st>>>(e, uvab, (float*)ctx->partials.p,
-                                                            ctx->g, ctx->layers[l], tvec_edge, write_e,
+                                                            ctx->g, ctx->layers[l], tvec_edge, tr, write_e,
                                                             ctx->agg_mode);
     CKL(ctx);
   } else {
     if (tc_launch_edge_layer(&ctx->tc, l, e, uvab, (float*)ctx->partials.p, ctx->g, ctx->layers[l],
-                             tvec_edge, write_e, e_zero, xt_for_lut, ctx->lut, ctx->agg_mode, impl.nwg,
+                             tvec_edge, tr, write_e, e_zero, xt_for_lut, ctx->lut, ctx->agg_mode, impl.nwg,
                              ctx->phase_timing, nullptr, st))
       FAIL(ctx, DFB_E_CUDA, "tensor-core edge layer: %s", ctx->tc.err.c_str());
     ctx->launches++;
@@ -749,12 +749,13 @@ static int launch_edge_layer(dfb_ctx* ctx, int l, float* e, const float* uvab, c
 
 // GNN layer l of the loaded model on the prepared graph, in place on h (V,256) and e (E,256, row-sorted), as
 // gnn_encoder.py:442-449 runs it: the node linears of h, the fused edge layer, then the node update.  tv is the layer's
-// time vector (on edges for TSP, on nodes for MIS).  Layer 0 of a forward passes its step-invariant inputs: uv0, TSP's
+// time vector (on edges for TSP, on nodes for MIS); with tr.index, the layer's vector of timestep 0, each element adding
+// its own timestep's.  Layer 0 of a forward passes its step-invariant inputs: uv0, TSP's
 // node linears of h0 (dfb_set_points), instead of computing them; e_zero (MIS: e0 = 0) or xt_lut (categorical TSP:
 // e0 read from the 2-row LUT) instead of reading e.  The last TSP layer skips the node update (TSP never reads h
 // after it, gnn_encoder.py:400) and the last MIS layer does not write e (gnn_encoder.py:412).
-static int run_layer(dfb_ctx* ctx, int l, float* h, float* e, const float* uv0, const float* tv, int e_zero,
-                     const float* xt_lut, cudaStream_t st) {
+static int run_layer(dfb_ctx* ctx, int l, float* h, float* e, const float* uv0, const float* tv, const TimeRows& tr,
+                     int e_zero, const float* xt_lut, cudaStream_t st) {
   const int L = ctx->L;
   const float* uv = uv0;
   if (!uv) {
@@ -763,12 +764,12 @@ static int run_layer(dfb_ctx* ctx, int l, float* h, float* e, const float* uv0, 
     uv = (const float*)ctx->uvab.p;
   }
   const int write_e = !(ctx->node_only && l == L - 1);
-  int r = launch_edge_layer(ctx, l, e, uv, ctx->node_only ? nullptr : tv, write_e, e_zero, xt_lut, st);
+  int r = launch_edge_layer(ctx, l, e, uv, ctx->node_only ? nullptr : tv, tr, write_e, e_zero, xt_lut, st);
   if (r) return r;
   if (ctx->node_only || l < L - 1) {
     k_node_update<<<(ctx->g.V + 7) / 8, 256, 0, st>>>(h, uv, (const float*)ctx->partials.p, ctx->g,
                                                       ctx->layers[l].ln_h_g, ctx->layers[l].ln_h_b,
-                                                      ctx->node_only ? tv : nullptr, ctx->agg_mode);
+                                                      ctx->node_only ? tv : nullptr, tr, ctx->agg_mode);
     CKL(ctx);
   }
   return DFB_OK;
@@ -816,11 +817,13 @@ static int run_entry(dfb_ctx* ctx, int mode, const float* xt, const float** xt_l
   return DFB_OK;
 }
 
-// Layer l of a forward at time vectors tvec [L][256]: layer 0 takes run_entry's step-invariant inputs.
-static int run_forward_layer(dfb_ctx* ctx, int l, const float* tvec, const float* xt_lut, int e_zero, cudaStream_t st) {
+// Layer l of a forward at time vectors tvec [L][256] (or, with tr.index, per element): layer 0 takes run_entry's
+// step-invariant inputs.
+static int run_forward_layer(dfb_ctx* ctx, int l, const float* tvec, const TimeRows& tr, const float* xt_lut,
+                             int e_zero, cudaStream_t st) {
   const bool first = l == 0;
   return run_layer(ctx, l, (float*)ctx->h.p, (float*)ctx->e.p,
-                   (first && !ctx->node_only) ? (const float*)ctx->uvab0.p : nullptr, tvec + (size_t)l * H,
+                   (first && !ctx->node_only) ? (const float*)ctx->uvab0.p : nullptr, tvec + (size_t)l * H, tr,
                    first ? e_zero : 0, first ? xt_lut : nullptr, st);
 }
 
@@ -842,17 +845,18 @@ static int run_head(dfb_ctx* ctx, int mode, const StepParams* sp, const float* Z
   return DFB_OK;
 }
 
-// Forward + head (mode HEAD_*) of step i of the staged tables: time vectors tvec[i], posterior parameters and output
-// pointers d_steps[i].  xt is the network input and the posterior's state in, xt_out its state out.
+// Forward + head (mode HEAD_*) of step i of the staged tables: time vectors tvec[i] (tr.index: element k at
+// tvec[i + tr.index[k]]), posterior parameters and output pointers d_steps[i].  xt is the network input and the
+// posterior's state in, xt_out its state out.
 static int run_forward(dfb_ctx* ctx, int mode, int i, const float* xt, float* xt_out, const float* uniforms,
-                       cudaStream_t st) {
+                       const TimeRows& tr, cudaStream_t st) {
   const float* tvec = (const float*)ctx->tvec.p + (size_t)i * ctx->L * H;
   const float* xt_lut;
   int e_zero;
   int r = run_entry(ctx, mode, xt, &xt_lut, &e_zero, st);
   if (r) return r;
   for (int l = 0; l < ctx->L; ++l) {
-    r = run_forward_layer(ctx, l, tvec, xt_lut, e_zero, st);
+    r = run_forward_layer(ctx, l, tvec, tr, xt_lut, e_zero, st);
     if (r) return r;
   }
   return run_head(ctx, mode, ctx->d_steps + i, ctx->node_only ? (const float*)ctx->h.p : (const float*)ctx->e.p, xt,
@@ -881,20 +885,41 @@ static int stage_commit(dfb_ctx* ctx, int slot, int n, cudaStream_t st) {
   return DFB_OK;
 }
 
-extern "C" int dfb_encoder_forward(dfb_ctx* ctx, const float* xt, float t, float* out, void* stream_) {
+// The n_t timesteps go through the step tables like a loop's: their time vectors are rows 0 .. n_t - 1 of tvec, and
+// with t_index row n_t is filled with NaN for the indices outside [0, n_t) (TimeRows).
+extern "C" int dfb_encoder_forward_timesteps(dfb_ctx* ctx, const float* xt, int n_t, const float* t_values,
+                                             const int32_t* t_index, float* out, void* stream_) {
   if (!ctx) return DFB_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream_;
   CK(ctx, cudaSetDevice(ctx->device));
   if (!ctx->graph_ready) FAIL(ctx, DFB_E_INVALID, "dfb_prepare_graph must be called first");
+  if (!t_values) FAIL(ctx, DFB_E_INVALID, "t_values is required");
+  if (n_t < 1) FAIL(ctx, DFB_E_INVALID, "n_t %d < 1", n_t);
+  if (n_t > dfb_ctx::MAX_STEPS)
+    FAIL(ctx, DFB_E_UNSUPPORTED, "%d distinct timesteps in one call: at most %d", n_t, dfb_ctx::MAX_STEPS);
+  if (t_index && !is_device_ptr(t_index)) FAIL(ctx, DFB_E_INVALID, "t_index must be a device pointer");
   int slot;
   int r = stage_acquire(ctx, &slot);
   if (r) return r;
-  ctx->h_tvals[slot][0] = t;
-  ctx->h_steps[slot][0] = StepParams{};
+  for (int i = 0; i < n_t; ++i) {
+    ctx->h_tvals[slot][i] = t_values[i];
+    ctx->h_steps[slot][i] = StepParams{};
+  }
   ctx->h_steps[slot][0].rec_out = out;
-  r = stage_commit(ctx, slot, 1, st);
+  const size_t layer_rows = (size_t)ctx->L * H;
+  if (t_index) ENS(ctx, ctx->tvec, (size_t)(n_t + 1) * layer_rows * sizeof(float));
+  r = stage_commit(ctx, slot, n_t, st);
   if (r) return r;
-  return run_forward(ctx, HEAD_FORWARD, 0, xt, nullptr, nullptr, st);
+  TimeRows tr{};
+  if (t_index) {
+    CK(ctx, cudaMemsetAsync((float*)ctx->tvec.p + (size_t)n_t * layer_rows, 0xff, layer_rows * sizeof(float), st));
+    tr = TimeRows{t_index, n_t, (int)layer_rows};
+  }
+  return run_forward(ctx, HEAD_FORWARD, 0, xt, nullptr, nullptr, tr, st);
+}
+
+extern "C" int dfb_encoder_forward(dfb_ctx* ctx, const float* xt, float t, float* out, void* stream_) {
+  return dfb_encoder_forward_timesteps(ctx, xt, 1, &t, nullptr, out, stream_);
 }
 
 // the head's posterior for a diffusion type, which the loaded head's out_channels must fit
@@ -936,14 +961,14 @@ extern "C" int dfb_denoise_step(dfb_ctx* ctx, int diffusion_type, const float* x
   if (mode == HEAD_CATEGORICAL) sp.rec_p = p_out;   // gaussian has no p: its p_out is left untouched
   r = stage_commit(ctx, slot, 1, st);
   if (r) return r;
-  return run_forward(ctx, mode, 0, xt_in, xt_out, uniforms, st);
+  return run_forward(ctx, mode, 0, xt_in, xt_out, uniforms, TimeRows{}, st);
 }
 
 // the `steps` forwards + posteriors of the loop, every per-step quantity read from device tables
 static int enqueue_loop(dfb_ctx* ctx, int mode, float* xt, int steps, const float* uniforms, cudaStream_t st) {
   const size_t N = ctx->node_only ? ctx->g.V : ctx->g.E;
   for (int i = 0; i < steps; ++i) {
-    int r = run_forward(ctx, mode, i, xt, xt, uniforms ? uniforms + (size_t)i * N : nullptr, st);
+    int r = run_forward(ctx, mode, i, xt, xt, uniforms ? uniforms + (size_t)i * N : nullptr, TimeRows{}, st);
     if (r) return r;
   }
   return DFB_OK;
@@ -1153,7 +1178,7 @@ extern "C" int dfb_debug_edge_gemm(dfb_ctx* ctx, int layer, const float* e_in, f
   if (!ctx->graph_ready) FAIL(ctx, DFB_E_INVALID, "dfb_prepare_graph must be called first");
   if (layer < 0 || layer >= ctx->L) FAIL(ctx, DFB_E_INVALID, "layer out of range");
   if (tc_launch_edge_layer(&ctx->tc, layer, const_cast<float*>(e_in), (const float*)ctx->uvab.p,
-                           (float*)ctx->partials.p, ctx->g, ctx->layers[layer], nullptr, 0, 0, nullptr, ctx->lut, AGG_SUM,
+                           (float*)ctx->partials.p, ctx->g, ctx->layers[layer], nullptr, TimeRows{}, 0, 0, nullptr, ctx->lut, AGG_SUM,
                            edge_impl(ctx).nwg, false, acc_out, st))
     FAIL(ctx, DFB_E_CUDA, "tensor-core edge layer: %s", ctx->tc.err.c_str());
   ctx->launches++;
@@ -1179,7 +1204,8 @@ extern "C" int dfb_debug_gnn_layer(dfb_ctx* ctx, int layer, float t, float* h, f
   ctx->h_steps[slot][0] = StepParams{};
   r = stage_commit(ctx, slot, 1, st);
   if (r) return r;
-  return run_layer(ctx, layer, h, e, nullptr, (const float*)ctx->tvec.p + (size_t)layer * H, 0, nullptr, st);
+  return run_layer(ctx, layer, h, e, nullptr, (const float*)ctx->tvec.p + (size_t)layer * H, TimeRows{}, 0, nullptr,
+                   st);
 }
 
 // Test hook: the head of a forward (run_head) on the caller's z, with one step row staged as dfb_denoise_step stages it.
@@ -1263,7 +1289,7 @@ extern "C" int dfb_debug_entry(dfb_ctx* ctx, int diffusion_type, const float* xt
     CK(ctx, cudaMemcpyAsync(e0_out, ctx->e.p, E * row, cudaMemcpyDeviceToDevice, st));
   }
   if (tvec_out) CK(ctx, cudaMemcpyAsync(tvec_out, ctx->tvec.p, ctx->L * row, cudaMemcpyDeviceToDevice, st));
-  r = run_forward_layer(ctx, 0, (const float*)ctx->tvec.p, xt_lut, e_zero, st);
+  r = run_forward_layer(ctx, 0, (const float*)ctx->tvec.p, TimeRows{}, xt_lut, e_zero, st);
   if (r) return r;
   if (h_out) CK(ctx, cudaMemcpyAsync(h_out, ctx->h.p, V * row, cudaMemcpyDeviceToDevice, st));
   if (e_out) CK(ctx, cudaMemcpyAsync(e_out, ctx->e.p, E * row, cudaMemcpyDeviceToDevice, st));

@@ -6,7 +6,7 @@
 // One block = one aggregation group of 32 row-sorted edges; thread = channel.
 //   e_hat = A h[col] + B h[row] + C e (+ b_C folded into B's bias)          gnn_encoder.py:104,110
 //   partial[group,node] = sum_{edges of node in group} sigmoid(e_hat) * V h[col]   :112,163,177-191
-//   e_til = relu(LN_e(e_hat)) (+ time vector, TSP)                            :131,135,445
+//   e_til = relu(LN_e(e_hat)) (+ time vector, TSP; with tr.index the edge's own)  :131,135,445
 //   e     = e + O(silu(LN_O(e_til))) + b_O                                     :449, :339-347
 #pragma once
 #include "common.cuh"
@@ -37,7 +37,7 @@ __device__ __forceinline__ void ef_tile_matvec(const float (*xs)[H], const float
 __global__ void __launch_bounds__(256) k_edge_layer_fp32(float* __restrict__ e, const float* __restrict__ uvab,
                                                          float* __restrict__ partials, GraphDev g,
                                                          LayerParams lp, const float* __restrict__ tvec_edge,
-                                                         int write_e, int agg_mode) {
+                                                         TimeRows tr, int write_e, int agg_mode) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float (*X)[H] = reinterpret_cast<float (*)[H]>(smem_raw);
   float (*Y)[H] = reinterpret_cast<float (*)[H]>(smem_raw + EF_ROWS * H * sizeof(float));
@@ -91,6 +91,8 @@ __global__ void __launch_bounds__(256) k_edge_layer_fp32(float* __restrict__ e, 
     int w = c >> 5, lane = c & 31;
     for (int rr = 0; rr < 4; ++rr) {
       int r = w * 4 + rr;
+      const float* tv = tvec_edge;
+      if (tv && tr.index && r < nrows) tv = time_row(tv, tr, g.perm ? g.perm[s0 + r] : s0 + r);
       float v[8];
       float s = 0.f;
 #pragma unroll
@@ -105,7 +107,7 @@ __global__ void __launch_bounds__(256) k_edge_layer_fp32(float* __restrict__ e, 
       for (int j = 0; j < 8; ++j) {
         int ch = lane + 32 * j;
         float y = fmaxf(fmaf((v[j] - mean) * rstd, lp.ln_e_g[ch], lp.ln_e_b[ch]), 0.0f);
-        if (tvec_edge) y += tvec_edge[ch];
+        if (tv) y += tv[ch];
         v[j] = y;
         s += y;
       }

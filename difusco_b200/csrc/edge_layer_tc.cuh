@@ -2,7 +2,7 @@
 //
 //   e_hat = C e + A h[col] + B h[row]                         gnn_encoder.py:104,110
 //   agg  += sigmoid(e_hat) * V h[col]   (row-segment sums)     :112,163,177-191
-//   e_til = relu(LN_e(e_hat)) + tau                            :131,135,445
+//   e_til = relu(LN_e(e_hat)) + tau                            :131,135,445   (tau per edge: k_edge_layer_wg*_trows)
 //   e     = e + O silu(LN_O(e_til)) + b_O   (in place)         :449, :339-347
 //
 // Persistent CTAs, one per SM, each looping over tiles of 64 * NWG row-sorted edges.
@@ -73,7 +73,10 @@ struct TcCfg {
   static constexpr int OFF_BAR = OFF_SRC + TILE * 8;
   static constexpr int SMEM_BYTES = OFF_BAR + 2 * NSTAGE * 8;
   static constexpr int SMEM_ALLOC = SMEM_BYTES + 1024;          // slack for 1024-byte alignment
-  static_assert(SMEM_ALLOC <= 232448, "shared memory budget (227 KB per block)");
+  // per-row time vectors (k_edge_layer_wg*_trows): each row's tau pointer, in a table past the product kernel's layout
+  static constexpr int OFF_TAU = SMEM_BYTES;
+  static constexpr int SMEM_ALLOC_TROWS = SMEM_ALLOC + TILE * 8;
+  static_assert(SMEM_ALLOC_TROWS <= 232448, "shared memory budget (227 KB per block)");
 };
 
 struct TcParams {
@@ -100,6 +103,7 @@ struct TcParams {
   int write_e, e_zero, agg_mode;
   int w_row_base;         // arena row of this layer's C (w_row_C)
   int n_tiles;
+  TimeRows trows;         // k_edge_layer_wg*_trows: tvec is the layer's row of timestep 0, edge s adds its own row
 };
 
 // ----------------------------------------------------------------------------------------------
@@ -273,8 +277,8 @@ enum {
 // and linear mode is a separate instantiation.  tests/test_kernel_footprint.py holds k_edge_layer_wg2 to its budget.
 // ----------------------------------------------------------------------------------------------
 // LIN selects linear mode (k_linear_wg2); TIMED adds the phase timers (clock reads pin instruction order, so the product
-// entry points are built without).
-template <int NWG, bool LIN, bool TIMED = false>
+// entry points are built without); TROWS reads tau per row, through P.trows, instead of one vector for every row.
+template <int NWG, bool LIN, bool TIMED = false, bool TROWS = false>
 __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, const TcParams& P) {
   using Cfg = TcCfg<NWG>;
   constexpr int NSTAGE = Cfg::NSTAGE;
@@ -283,6 +287,7 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
   float* prm = reinterpret_cast<float*>(smem + Cfg::OFF_PRM);
   int* s_row = reinterpret_cast<int*>(smem + Cfg::OFF_ROW);
   const float** s_src = reinterpret_cast<const float**>(smem + Cfg::OFF_SRC);
+  const float** s_tau = reinterpret_cast<const float**>(smem + Cfg::OFF_TAU);   // TROWS only
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);   // [NSTAGE] TMA -> consumers (expect_tx)
   uint64_t* empty = full + NSTAGE;                                      // [NSTAGE] the 4 reading warps -> producer
 
@@ -341,6 +346,7 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
   float* msg = reinterpret_cast<float*>(a_reg);   // [64][256] fp32, column c of row r at c ^ 8 (r & 7)
   int* w_row = s_row + wg * WG_ROWS;
   const float** w_src = s_src + wg * WG_ROWS;
+  const float** w_tau = s_tau + wg * WG_ROWS;
   auto wg_bar = [&] { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); };
   const int n_rows = lin ? P.lin_rows : P.g.E;
   // Chunks this warpgroup has read.  With two consumer warpgroups the ring also carries the other warpgroup's 8 chunks
@@ -447,6 +453,7 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
       }
       w_row[tid] = rw;
       w_src[tid] = src;
+      if constexpr (TROWS) w_tau[tid] = s < n_rows ? time_row(P.tvec, P.trows, P.g.perm ? P.g.perm[s] : s) : P.zero_row;
     }
     wg_bar();   // row table visible; every warp has left the previous tile's GEMM2 (A operand area free)
 
@@ -581,12 +588,16 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
       }
       float rstd = rsqrtf(quad_sum(q) * (1.0f / H) + LN_EPS);
       sum = 0.f;
+      const float* tau = nullptr;
+      if constexpr (TROWS) tau = w_tau[lr0 + 8 * h];
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         const int c = 8 * j + 2 * t4;
         const float2 g = *reinterpret_cast<const float2*>(prm + c);
         const float2 b = *reinterpret_cast<const float2*>(prm + H + c);
-        const float2 t = *reinterpret_cast<const float2*>(prm + 2 * H + c);
+        float2 t;
+        if constexpr (TROWS) t = __ldg(reinterpret_cast<const float2*>(tau + c));
+        else t = *reinterpret_cast<const float2*>(prm + 2 * H + c);
         const float y0 = fmaxf(fmaf((acc[4 * j] - mean) * rstd, g.x, b.x), 0.0f) + t.x;
         const float y1 = fmaxf(fmaf((acc[4 * j + 1] - mean) * rstd, g.y, b.y), 0.0f) + t.y;
         acc[4 * j] = y0;
@@ -666,6 +677,16 @@ __global__ void __launch_bounds__(TcCfg<1>::THREADS, 1)
 k_edge_layer_wg1(const __grid_constant__ CUtensorMap wmap, const TcParams P) {
   edge_layer_wg_body<1, false>(wmap, P);
 }
+// the two edge kernels with a timestep per edge (dfb_encoder_forward_timesteps), launched only when the call has one:
+// the product kernels keep reading tau from shared memory
+__global__ void __launch_bounds__(TcCfg<2>::THREADS, 1)
+k_edge_layer_wg2_trows(const __grid_constant__ CUtensorMap wmap, const TcParams P) {
+  edge_layer_wg_body<2, false, false, true>(wmap, P);
+}
+__global__ void __launch_bounds__(TcCfg<1>::THREADS, 1)
+k_edge_layer_wg1_trows(const __grid_constant__ CUtensorMap wmap, const TcParams P) {
+  edge_layer_wg_body<1, false, false, true>(wmap, P);
+}
 // the same body in linear mode (node-side / embedding linears) under its own name, so launch lists and profiles
 // do not mix the two uses; the edge kernels carry none of its code
 __global__ void __launch_bounds__(TcCfg<2>::THREADS, 1)
@@ -708,6 +729,10 @@ inline int tc_init(TcState* st, int num_sms) {
     e = cudaFuncSetAttribute(k_edge_layer_wg2_timed, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<2>::SMEM_ALLOC);
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute(k_edge_layer_wg1, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<1>::SMEM_ALLOC);
+  if (e == cudaSuccess)
+    e = cudaFuncSetAttribute(k_edge_layer_wg2_trows, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<2>::SMEM_ALLOC_TROWS);
+  if (e == cudaSuccess)
+    e = cudaFuncSetAttribute(k_edge_layer_wg1_trows, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<1>::SMEM_ALLOC_TROWS);
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute(k_linear_wg2, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<2>::SMEM_ALLOC);
   if (e != cudaSuccess) {
@@ -756,7 +781,7 @@ inline int tc_bind_weights(TcState* st, const uint16_t* arena, int L) {
 // per SM, fewer when there are fewer tiles.  P holds the launch's own arguments; the context's are added here.
 template <int NWG>
 inline int tc_launch(TcState* st, void (*kernel)(CUtensorMap, TcParams), TcParams& P, int rows, int nb,
-                     cudaStream_t stream) {
+                     cudaStream_t stream, int smem = TcCfg<NWG>::SMEM_ALLOC) {
   if (!st->bound) {
     st->err = "weights not bound";
     return -1;
@@ -764,7 +789,7 @@ inline int tc_launch(TcState* st, void (*kernel)(CUtensorMap, TcParams), TcParam
   P.zero_row = st->zero_row; P.error_flag = st->error_flag; P.phase_cycles = st->phase_cycles;
   P.n_tiles = nb * ((rows + TcCfg<NWG>::TILE - 1) / TcCfg<NWG>::TILE);
   const int grid = P.n_tiles < st->num_sms ? P.n_tiles : st->num_sms;
-  kernel<<<grid, TcCfg<NWG>::THREADS, TcCfg<NWG>::SMEM_ALLOC, stream>>>(st->wmap, P);
+  kernel<<<grid, TcCfg<NWG>::THREADS, smem, stream>>>(st->wmap, P);
   const cudaError_t err = cudaGetLastError();
   if (err == cudaSuccess) return 0;
   st->err = std::string("launch: ") + cudaGetErrorString(err);
@@ -773,17 +798,24 @@ inline int tc_launch(TcState* st, void (*kernel)(CUtensorMap, TcParams), TcParam
 
 // One fused edge layer l over graph g.  nwg 2: k_edge_layer_wg2, the product kernel, or with `timed` its copy with
 // phase timers, k_edge_layer_wg2_timed; nwg 1: k_edge_layer_wg1, the 64-row-tile variant.  A non-null debug_acc
-// (tests) runs GEMM1 only and writes its accumulator [E][256] there, never through the timed copy.
+// (tests) runs GEMM1 only and writes its accumulator [E][256] there, never through the timed copy.  With a non-null
+// trows.index (a TSP layer with a timestep per edge) the launch goes to k_edge_layer_wg<nwg>_trows, which has no
+// phase timers.
 inline int tc_launch_edge_layer(TcState* st, int l, float* e, const float* uvab, float* partials, const GraphDev& g,
-                                const LayerParams& lp, const float* tvec, int write_e, int e_zero, const float* xt_lut,
-                                const float* lut, int agg_mode, int nwg, bool timed, float* debug_acc,
-                                cudaStream_t stream) {
+                                const LayerParams& lp, const float* tvec, const TimeRows& trows, int write_e,
+                                int e_zero, const float* xt_lut, const float* lut, int agg_mode, int nwg, bool timed,
+                                float* debug_acc, cudaStream_t stream) {
   TcParams P{};
   P.e = e; P.uvab = uvab; P.partials = partials; P.g = g; P.lp = lp; P.tvec = tvec;
   P.xt_lut = xt_lut; P.lut = lut; P.debug_acc = debug_acc;
   P.write_e = debug_acc ? 0 : write_e;
   P.e_zero = e_zero; P.agg_mode = agg_mode;
   P.w_row_base = w_row_C(l);
+  if (trows.index && tvec && !debug_acc) {
+    P.trows = trows;
+    if (nwg == 1) return tc_launch<1>(st, k_edge_layer_wg1_trows, P, g.E, 1, stream, TcCfg<1>::SMEM_ALLOC_TROWS);
+    return tc_launch<2>(st, k_edge_layer_wg2_trows, P, g.E, 1, stream, TcCfg<2>::SMEM_ALLOC_TROWS);
+  }
   if (nwg == 1) return tc_launch<1>(st, k_edge_layer_wg1, P, g.E, 1, stream);
   return tc_launch<2>(st, timed && !debug_acc ? k_edge_layer_wg2_timed : k_edge_layer_wg2, P, g.E, 1, stream);
 }

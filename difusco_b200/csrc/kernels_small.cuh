@@ -135,16 +135,18 @@ __global__ void __launch_bounds__(256) k_linear(const float* __restrict__ X, con
 //   h[i] += relu(LN_h(Uh[i] + sum_{edges of i} gate*Vh)) (+ tvec for MIS, :447)
 // The aggregated messages arrive as per-(group,node) partial sums written by the edge kernel;
 // they are added in ascending group order -> bitwise deterministic, no atomics.
-// One warp per node, lane owns 8 channels.
+// One warp per node, lane owns 8 channels.  With tr.index, node i adds its own timestep's row of tvec.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_node_update(float* __restrict__ h, const float* __restrict__ uvab,
                                                      const float* __restrict__ partials, GraphDev g,
                                                      const float* __restrict__ ln_g,
                                                      const float* __restrict__ ln_b,
-                                                     const float* __restrict__ tvec_or_null, int agg_mode) {
+                                                     const float* __restrict__ tvec_or_null, TimeRows tr,
+                                                     int agg_mode) {
   int i = blockIdx.x * 8 + (threadIdx.x >> 5);
   int lane = threadIdx.x & 31;
   if (i >= g.V) return;
+  if (tvec_or_null && tr.index) tvec_or_null = time_row(tvec_or_null, tr, i);
   float x[8];
   {
     const float4* u = reinterpret_cast<const float4*>(uvab + (size_t)i * 4 * H) + lane * 2;

@@ -8,19 +8,23 @@ math: it hands raw device pointers to the sm_100a CUDA library through the C-ABI
 the call raises.
 
 Interface notes (reference behaviour kept):
-  * sparse TSP  : forward(x (V,2), t (1,), graph=xt (E,), edge_index (2,E)) -> (E, out)    :383-402
-  * MIS         : forward(xt (V,), t (1,), edge_index=(2,E))              -> (V, out)      :404-414
-  * dense TSP   : forward(x (B,V,2), t (B,), graph=xt (B,V,V))            -> (B,out,V,V)   :350-381
+  * sparse TSP  : forward(x (V,2), t (1,) or (E,), graph=xt (E,), edge_index (2,E)) -> (E, out)    :383-402
+  * MIS         : forward(xt (V,), t (1,) or (V,), edge_index=(2,E))               -> (V, out)      :404-414
+  * dense TSP   : forward(x (B,V,2), t (1,) or (B,), graph=xt (B,V,V))             -> (B,out,V,V)   :350-381
     evaluated as the row-major complete graph incl. self pairs (gnn_encoder.py:365 makes the
-    graph all-ones), GroupNorm per sample.
+    graph all-ones), GroupNorm per sample, in one call whatever the timesteps.
+  * a timestep per element (the reference's training steps, pl_tsp_model.py:66-67, pl_mis_model.py:54) runs in the
+    same single call (dfb_encoder_forward_timesteps); with use_activation_checkpoint=True the sparse forwards run
+    every element at t[0], as the reference's checkpointed branch does (gnn_encoder.py:429).  The sparse forwards read
+    different per-element timesteps on the model's device, where the training steps put them; a host tensor of them
+    raises NotImplementedError.
   * dense + node_feature_only raises NotImplementedError (:457), as in the reference.
   * sparse TSP and MIS take a keyword-only node_ptr (PyG's Batch.ptr: instance i owns nodes
     [node_ptr[i], node_ptr[i+1])): one block-diagonal call over a ragged batch whose head GroupNorm
     runs per instance, so every instance gets the result it would get alone (the reference's test
     loader runs batch size 1).  Without it the GroupNorm statistics span every row of the call.
-Only inference is in scope: per-edge timestep vectors (training, pl_tsp_model.py:66-68) raise
-NotImplementedError; autograd is not supported - outputs carry no grad_fn, and a call with grad mode
-enabled on parameters that require grad warns once.
+Only the forward is in scope: autograd is not supported - outputs carry no grad_fn, and a call with grad mode enabled
+on parameters that require grad warns once.  A training-step loss is evaluated under torch.no_grad().
 """
 import math
 
@@ -42,6 +46,36 @@ def reference_frequency_tables(hidden_dim):
   dimt_scalar = 10000 ** (2 * torch.div(i, 2, rounding_mode="trunc") / hidden_dim)
   return {"__const.time_freqs": freqs.numpy(), "__const.dimt_pos": dimt_pos.numpy(),
           "__const.dimt_scalar": dimt_scalar.numpy()}
+
+
+MAX_TIMESTEPS = 4096   # distinct timesteps of one call (the device step table of dfb_encoder_forward_timesteps)
+
+
+def timestep_args(timesteps, n, first_only=False, device=None):
+  """The timesteps of a forward over n elements (edges, nodes or dense samples) -> a float, the one timestep of the
+  call, or (values, index): the distinct timesteps as a host float32 array and, on the device of `timesteps`, each
+  element's position among them as int32 (n,).  One value, or n equal values, give the float.  first_only (the
+  reference's checkpointed sparse layers, gnn_encoder.py:429) gives t[0] for any length.  With `device` (the sparse
+  forwards), different timesteps must lie on it, where the reference's training steps put them
+  (pl_tsp_model.py:76-81, pl_mis_model.py:65-69): a host tensor of them raises NotImplementedError, as every
+  per-element call of the sparse forwards did before they were supported."""
+  t = timesteps.reshape(-1).float()
+  if t.numel() == 0 or (t.numel() not in (1, n) and not first_only):
+    raise ValueError(f"timesteps must hold 1 or {n} values (one per element), got {t.numel()}")
+  if t.numel() == 1:
+    return float(t[0])
+  if device is not None and t.device != torch.device(device) and not bool((t == t[0]).all()):
+    raise NotImplementedError(f"different timesteps per element are read on the model's device ({device}), where "
+                              f"the reference's training steps put them; got a {t.device} tensor")
+  if first_only:
+    return float(t[0])
+  values, index = torch.unique(t, return_inverse=True)
+  if values.numel() == 1:
+    return float(values[0])
+  if values.numel() > MAX_TIMESTEPS:
+    raise NotImplementedError(f"{values.numel()} distinct timesteps in one forward; at most {MAX_TIMESTEPS} are "
+                              "supported (integer timesteps in [1, T] never exceed it)")
+  return values.cpu().numpy(), index.to(torch.int32)
 
 
 def node_ptr_array(node_ptr):
@@ -94,7 +128,9 @@ class GNNEncoder(nn.Module):
     self.n_layers = n_layers
     self.out_channels = out_channels
     self.aggregation = aggregation
-    self.use_activation_checkpoint = use_activation_checkpoint   # training-only memory knob: ignored
+    # a training memory knob; the reference's checkpointed sparse layers run every element at t[0] (gnn_encoder.py:429),
+    # which the sparse forwards reproduce.  The dense forward ignores it (the reference raises there, :370-371).
+    self.use_activation_checkpoint = use_activation_checkpoint
     ted = hidden_dim // 2
     self.node_embed = nn.Linear(hidden_dim, hidden_dim)
     self.edge_embed = nn.Linear(hidden_dim, hidden_dim)
@@ -195,50 +231,53 @@ class GNNEncoder(nn.Module):
       self._complete_cache[key] = torch.stack([r.repeat(B) + off, c.repeat(B) + off]).long().contiguous()
     return self._complete_cache[key]
 
-  @staticmethod
-  def _single_t(timesteps):
-    t = timesteps.reshape(-1).float()
-    if t.numel() != 1 and not bool((t == t[0]).all()):
-      raise NotImplementedError("per-element timesteps (the training path) are outside difusco_b200's scope")
-    return float(t[0])
+  def _run(self, ctx, xt, t, out):
+    """One forward at t: a float (dfb_encoder_forward) or timestep_args' (values, index)."""
+    if isinstance(t, float):
+      ctx.encoder_forward(xt.data_ptr(), t, out.data_ptr(), self._stream())
+      return
+    values, index = t
+    index = index.to(self._device()).contiguous()
+    ctx.encoder_forward_timesteps(xt.data_ptr(), values, index.data_ptr(), out.data_ptr(), self._stream())
 
   # ------------------------------------------------------------------------------------------
   # forward variants (gnn_encoder.py:350-462)
   # ------------------------------------------------------------------------------------------
   def sparse_forward(self, x, graph, timesteps, edge_index, node_ptr=None):
     V, E = x.shape[0], edge_index.shape[1]
+    t = timestep_args(timesteps, E, self.use_activation_checkpoint, self.node_embed.weight.device)
     ctx = self.set_graph(edge_index, V, 1, node_ptr)
     self.set_points(x.to(self._device()))
     xt = graph.reshape(-1).float().contiguous().to(self._device())
     out = torch.empty((E, self.out_channels), device=self._device(), dtype=torch.float32)
-    ctx.encoder_forward(xt.data_ptr(), self._single_t(timesteps), out.data_ptr(), self._stream())
+    self._run(ctx, xt, t, out)
     return out
 
   def sparse_forward_node_feature_only(self, x, timesteps, edge_index, node_ptr=None):
     V = x.shape[0]
+    t = timestep_args(timesteps, V, self.use_activation_checkpoint, self.node_embed.weight.device)
     ctx = self.set_graph(edge_index, V, 1, node_ptr)
     xt = x.reshape(-1).float().contiguous().to(self._device())
     out = torch.empty((V, self.out_channels), device=self._device(), dtype=torch.float32)
-    ctx.encoder_forward(xt.data_ptr(), self._single_t(timesteps), out.data_ptr(), self._stream())
+    self._run(ctx, xt, t, out)
     return out
 
   def dense_forward(self, x, graph, timesteps, edge_index=None):
+    """One block-diagonal call over the B complete graphs, GroupNorm per sample (gn_segments = B); a timestep per
+    sample (:364, :375) indexes each sample's V * V edges."""
     del edge_index
     B, V, _ = x.shape
+    t = timestep_args(timesteps, B)
+    if not isinstance(t, float):
+      t = (t[0], t[1].repeat_interleave(V * V))
     dev = self._device()
-    t = timesteps.reshape(-1).float()
-    same_t = t.numel() == 1 or bool((t == t[0]).all())
     out = torch.empty((B, self.out_channels, V, V), device=dev, dtype=torch.float32)
-    if same_t:          # one block-diagonal call, GroupNorm per sample (gn_segments = B)
-      ctx = self.set_graph(self._complete_graph(B, V, dev), B * V, B)
-      self.set_points(x.reshape(B * V, 2).to(dev))
-      xt = graph.reshape(-1).float().contiguous().to(dev)
-      flat = torch.empty((B * V * V, self.out_channels), device=dev, dtype=torch.float32)
-      ctx.encoder_forward(xt.data_ptr(), float(t[0]), flat.data_ptr(), self._stream())
-      out.copy_(flat.reshape(B, V, V, self.out_channels).permute(0, 3, 1, 2))
-    else:               # different timestep per sample (dense_forward allows it, :375)
-      for b in range(B):
-        out[b:b + 1] = self.dense_forward(x[b:b + 1], graph[b:b + 1], t[b:b + 1])
+    ctx = self.set_graph(self._complete_graph(B, V, dev), B * V, B)
+    self.set_points(x.reshape(B * V, 2).to(dev))
+    xt = graph.reshape(-1).float().contiguous().to(dev)
+    flat = torch.empty((B * V * V, self.out_channels), device=dev, dtype=torch.float32)
+    self._run(ctx, xt, t, flat)
+    out.copy_(flat.reshape(B, V, V, self.out_channels).permute(0, 3, 1, 2))
     return out
 
   def forward(self, x, timesteps, graph=None, edge_index=None, *, node_ptr=None):

@@ -101,6 +101,21 @@ int dfb_set_points(dfb_ctx* ctx, const float* points, void* stream);
  * `t` is the (single) timestep, as at inference (pl_tsp_model.py:124-130). */
 int dfb_encoder_forward(dfb_ctx* ctx, const float* xt, float t, float* out, void* stream);
 
+/* GNNEncoder.forward with a timestep per element, as the reference's training steps call it (pl_tsp_model.py:66-67,
+ * pl_mis_model.py:54; gnn_encoder.py:396, :445, :447): the loss of a checkpoint as a function of t, under no_grad.
+ *   t_values  HOST (n_t,) fp32, 1 <= n_t <= 4096, the call's distinct timesteps
+ *   t_index   DEVICE (N,) int32 in the caller's element order (N = E for TSP, V for MIS): element i runs at
+ *             t_values[t_index[i]].  NULL: every element runs at t_values[0] (this is dfb_encoder_forward).
+ *   xt, out   as dfb_encoder_forward.
+ * A dense batch with a timestep per sample is the complete-graph call with t_index = the sample of each edge.
+ * An index outside [0, n_t) does not read out of bounds: its element gets a NaN time vector, which reaches the head
+ * GroupNorm statistics; the head's ReLU maps the NaN to 0, so every output row of the affected GroupNorm segments is
+ * the head's bias.  The call returns DFB_OK and the context stays usable.  No allocation beyond the first call of a
+ * size, no host synchronisation.  DFB_E_INVALID before any device work on a null t_values, n_t < 1 or a host t_index;
+ * DFB_E_UNSUPPORTED when n_t > 4096. */
+int dfb_encoder_forward_timesteps(dfb_ctx* ctx, const float* xt, int n_t, const float* t_values,
+                                  const int32_t* t_index, float* out, void* stream);
+
 /* One reverse-diffusion step = *_denoise_step (pl_tsp_model.py:122-151, pl_mis_model.py:118-140)
  * = forward + softmax + categorical_posterior (pl_meta_model.py:102-146) or gaussian_posterior
  * (:148-175), fused on the device.

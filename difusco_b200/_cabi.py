@@ -21,7 +21,7 @@ SYMBOLS = [
     "dfb_encoder_forward", "dfb_encoder_forward_timesteps", "dfb_denoise_step", "dfb_denoise", "dfb_denoise_record", "dfb_denoise_instances",
     "dfb_denoise_host",
     "dfb_launch_count", "dfb_profile_begin", "dfb_profile_end", "dfb_debug_edge_gemm", "dfb_debug_gnn_layer",
-    "dfb_debug_head", "dfb_debug_entry", "dfb_debug_loop_captures",
+    "dfb_debug_gnn_layer_timesteps", "dfb_debug_head", "dfb_debug_entry", "dfb_debug_loop_captures",
     "dfb_debug_phase_cycles", "dfb_debug_watchdog", "dfb_knn_graph", "dfb_set_graph_capture",
     "dfb_set_phase_timing", "dfb_tsp_merge_sparse", "dfb_tsp_merge_order", "dfb_two_opt", "dfb_two_opt_instances",
     "dfb_write_heatmap_txt",
@@ -71,6 +71,7 @@ def lib():
   L.dfb_profile_end.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(i64)]
   L.dfb_debug_edge_gemm.argtypes = [vp, i32, vp, vp, vp]
   L.dfb_debug_gnn_layer.argtypes = [vp, i32, f32, vp, vp, vp]
+  L.dfb_debug_gnn_layer_timesteps.argtypes = [vp, i32, i32, C.POINTER(f32), vp, vp, vp, vp]
   L.dfb_debug_head.argtypes = [vp, i32, vp, C.POINTER(f32), i32, vp, u64, i32, vp, vp, vp, vp, vp, vp, vp]
   L.dfb_debug_entry.argtypes = [vp, i32, vp, f32, vp, vp, vp, vp, vp, vp]
   L.dfb_debug_phase_cycles.argtypes = [vp, C.POINTER(C.c_uint64)]
@@ -399,6 +400,13 @@ class Context(object):
     """Run GNN layer `layer` alone at timestep t, in place on device h (V,256) and e (E,256); e rows in the prepared
     graph's stable row-sorted order."""
     self._ck(lib().dfb_debug_gnn_layer(self._h, int(layer), float(t), h_ptr, e_ptr, stream))
+
+  def debug_gnn_layer_timesteps(self, layer, t_values, t_index_ptr, h_ptr, e_ptr, stream=0):
+    """debug_gnn_layer with a timestep per element, as encoder_forward_timesteps runs each layer: t_values the distinct
+    timesteps (host sequence), t_index_ptr a device int32 (N,) array in the caller's element order, or None."""
+    v = np.ascontiguousarray(t_values, dtype=np.float32).reshape(-1)
+    self._ck(lib().dfb_debug_gnn_layer_timesteps(self._h, int(layer), v.size, v.ctypes.data_as(C.POINTER(C.c_float)),
+                                                 t_index_ptr, h_ptr, e_ptr, stream))
 
   def debug_head(self, mode, z_ptr, consts=(0, 0, 0, 0), last=0, uniforms_ptr=None, seed=0, step_index=0,
                  instance_seeds_ptr=None, xt_in_ptr=None, xt_out_ptr=None, p_out_ptr=None, net_out_ptr=None,

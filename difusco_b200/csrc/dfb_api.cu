@@ -885,13 +885,12 @@ static int stage_commit(dfb_ctx* ctx, int slot, int n, cudaStream_t st) {
   return DFB_OK;
 }
 
-// The n_t timesteps go through the step tables like a loop's: their time vectors are rows 0 .. n_t - 1 of tvec, and
-// with t_index row n_t is filled with NaN for the indices outside [0, n_t) (TimeRows).
-extern "C" int dfb_encoder_forward_timesteps(dfb_ctx* ctx, const float* xt, int n_t, const float* t_values,
-                                             const int32_t* t_index, float* out, void* stream_) {
-  if (!ctx) return DFB_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream_;
-  CK(ctx, cudaSetDevice(ctx->device));
+// The argument checks and staging of a call with a timestep per element (dfb_encoder_forward_timesteps,
+// dfb_debug_gnn_layer_timesteps).  The n_t timesteps go through the step tables like a loop's: their time vectors are
+// rows 0 .. n_t - 1 of tvec, and with t_index row n_t is filled with NaN for the indices outside [0, n_t) (TimeRows).
+// Every check comes before any device work; `out` is step 0's network output (rec_out), or null.  -> *tr
+static int stage_timesteps(dfb_ctx* ctx, int n_t, const float* t_values, const int32_t* t_index, float* out,
+                           TimeRows* tr, cudaStream_t st) {
   if (!ctx->graph_ready) FAIL(ctx, DFB_E_INVALID, "dfb_prepare_graph must be called first");
   if (!t_values) FAIL(ctx, DFB_E_INVALID, "t_values is required");
   if (n_t < 1) FAIL(ctx, DFB_E_INVALID, "n_t %d < 1", n_t);
@@ -910,11 +909,22 @@ extern "C" int dfb_encoder_forward_timesteps(dfb_ctx* ctx, const float* xt, int 
   if (t_index) ENS(ctx, ctx->tvec, (size_t)(n_t + 1) * layer_rows * sizeof(float));
   r = stage_commit(ctx, slot, n_t, st);
   if (r) return r;
-  TimeRows tr{};
+  *tr = TimeRows{};
   if (t_index) {
     CK(ctx, cudaMemsetAsync((float*)ctx->tvec.p + (size_t)n_t * layer_rows, 0xff, layer_rows * sizeof(float), st));
-    tr = TimeRows{t_index, n_t, (int)layer_rows};
+    *tr = TimeRows{t_index, n_t, (int)layer_rows};
   }
+  return DFB_OK;
+}
+
+extern "C" int dfb_encoder_forward_timesteps(dfb_ctx* ctx, const float* xt, int n_t, const float* t_values,
+                                             const int32_t* t_index, float* out, void* stream_) {
+  if (!ctx) return DFB_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream_;
+  CK(ctx, cudaSetDevice(ctx->device));
+  TimeRows tr;
+  int r = stage_timesteps(ctx, n_t, t_values, t_index, out, &tr, st);
+  if (r) return r;
   return run_forward(ctx, HEAD_FORWARD, 0, xt, nullptr, nullptr, tr, st);
 }
 
@@ -1187,25 +1197,26 @@ extern "C" int dfb_debug_edge_gemm(dfb_ctx* ctx, int layer, const float* e_in, f
 
 extern "C" int64_t dfb_debug_loop_captures(const dfb_ctx* ctx) { return ctx ? ctx->loop_captures : 0; }
 
-// Test hook: GNN layer `layer` alone (run_layer, the code run_forward runs for it) at timestep t, in place on the
-// caller's h (V,256) and e (E,256, row-sorted).  Always reads e and computes the node linears of h: never the LUT,
-// e_zero or the cached layer-0 node linears.
-extern "C" int dfb_debug_gnn_layer(dfb_ctx* ctx, int layer, float t, float* h, float* e, void* stream_) {
+// Test hook: GNN layer `layer` alone (run_layer, the code run_forward runs for it) with the time vectors of a call to
+// dfb_encoder_forward_timesteps, in place on the caller's h (V,256) and e (E,256, row-sorted); t_index in the caller's
+// element order, as the forward takes it.  Always reads e and computes the node linears of h: never the LUT, e_zero
+// or the cached layer-0 node linears.
+extern "C" int dfb_debug_gnn_layer_timesteps(dfb_ctx* ctx, int layer, int n_t, const float* t_values,
+                                             const int32_t* t_index, float* h, float* e, void* stream_) {
   if (!ctx) return DFB_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream_;
   CK(ctx, cudaSetDevice(ctx->device));
-  if (!ctx->graph_ready) FAIL(ctx, DFB_E_INVALID, "dfb_prepare_graph must be called first");
   if (layer < 0 || layer >= ctx->L) FAIL(ctx, DFB_E_INVALID, "layer %d out of range for %d layers", layer, ctx->L);
   if (!is_device_ptr(h) || !is_device_ptr(e)) FAIL(ctx, DFB_E_INVALID, "h and e must be device pointers");
-  int slot;
-  int r = stage_acquire(ctx, &slot);
+  TimeRows tr;
+  int r = stage_timesteps(ctx, n_t, t_values, t_index, nullptr, &tr, st);
   if (r) return r;
-  ctx->h_tvals[slot][0] = t;
-  ctx->h_steps[slot][0] = StepParams{};
-  r = stage_commit(ctx, slot, 1, st);
-  if (r) return r;
-  return run_layer(ctx, layer, h, e, nullptr, (const float*)ctx->tvec.p + (size_t)layer * H, TimeRows{}, 0, nullptr,
-                   st);
+  return run_layer(ctx, layer, h, e, nullptr, (const float*)ctx->tvec.p + (size_t)layer * H, tr, 0, nullptr, st);
+}
+
+// Test hook: the same at one timestep t for every element.
+extern "C" int dfb_debug_gnn_layer(dfb_ctx* ctx, int layer, float t, float* h, float* e, void* stream_) {
+  return dfb_debug_gnn_layer_timesteps(ctx, layer, 1, &t, nullptr, h, e, stream_);
 }
 
 // Test hook: the head of a forward (run_head) on the caller's z, with one step row staged as dfb_denoise_step stages it.

@@ -257,6 +257,15 @@ int dfb_debug_edge_gemm(dfb_ctx* ctx, int layer, const float* e_in, float* acc_o
  * MIS layer e is.  Always reads e and h: never the categorical LUT, the MIS e0 = 0 or the cached layer-0 linears. */
 int dfb_debug_gnn_layer(dfb_ctx* ctx, int layer, float t, float* h, float* e, void* stream);
 
+/* Test hook: dfb_debug_gnn_layer with a timestep per element, as dfb_encoder_forward_timesteps runs each layer:
+ * t_values, n_t and t_index as there (t_index DEVICE (N,) int32 in the caller's element order, NULL for every element at
+ * t_values[0]); h and e as dfb_debug_gnn_layer (e row-sorted).  An index outside [0, n_t) gives its element a NaN time
+ * vector: the NaN reaches that edge's row of e (TSP) or that node's row of h (MIS) and no other value of the layer.
+ * Same argument errors as both calls, before any device work.  dfb_debug_gnn_layer is this call with n_t = 1 and
+ * t_index = NULL. */
+int dfb_debug_gnn_layer_timesteps(dfb_ctx* ctx, int layer, int n_t, const float* t_values, const int32_t* t_index,
+                                  float* h, float* e, void* stream);
+
 /* Test hook: the head of a forward alone (GroupNorm statistics of each segment of the prepared graph, GroupNorm, ReLU,
  * 1x1 conv, then the posterior of `mode`, DFB_HEAD_*) on a DEVICE z (R,256) fp32: R = E rows in the prepared graph's
  * row-sorted order for TSP, V rows in node order for MIS.  The segment table, perm and per-instance rank table of the

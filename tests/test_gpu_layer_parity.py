@@ -125,15 +125,21 @@ def _engine(weights, task, n_layers=N_LAYERS):
   return _engines[key][0].engine()
 
 
-def _run_layer(ctx, ei, V, layer, h, e, impl, agg, t=T_LAYER):
-  """dfb_debug_gnn_layer on fp32 h (V,256) and e (E,256) in the caller's edge order -> (h_out, e_out), same order."""
+def _run_layer(ctx, ei, V, layer, h, e, impl, agg, t=T_LAYER, t_index=None):
+  """dfb_debug_gnn_layer on fp32 h (V,256) and e (E,256) in the caller's edge order -> (h_out, e_out), same order.
+  With t_index (int32, one per edge for TSP or per node for MIS, caller's order), dfb_debug_gnn_layer_timesteps with
+  t the sequence of distinct timesteps."""
   ctx.set_edge_impl(G.IMPLS[impl])
   ctx.set_aggregation(agg)
   eid = G.cu(ei)
   ctx.prepare_graph(eid.data_ptr(), V, ei.shape[1], 1, _stream())
   perm = np.argsort(ei[0], kind="stable")
   hd, ed = G.cu(np.asarray(h, np.float32)), G.cu(np.asarray(e, np.float32)[perm])
-  ctx.debug_gnn_layer(layer, t, hd.data_ptr(), ed.data_ptr(), _stream())
+  if t_index is None:
+    ctx.debug_gnn_layer(layer, t, hd.data_ptr(), ed.data_ptr(), _stream())
+  else:
+    idx = G.cu(np.asarray(t_index, np.int32))
+    ctx.debug_gnn_layer_timesteps(layer, t, idx.data_ptr(), hd.data_ptr(), ed.data_ptr(), _stream())
   torch.cuda.synchronize()
   e_out = np.empty_like(ed.cpu().numpy())
   e_out[perm] = ed.cpu().numpy()
@@ -157,14 +163,15 @@ def _check_layer(got_h, got_e, h_in, e_in, r64, r32, task, layer, n_layers, impl
   _assert_within(got, yard, impl, what)
 
 
-def _refs(weights, task, case, layer, h, e, agg):
-  """(fp64, fp32) oracle layer `layer` on the fp32 state (h, e), caller's edge order, as numpy."""
+def _refs(weights, task, case, layer, h, e, agg, t=(T_LAYER,)):
+  """(fp64, fp32) oracle layer `layer` on the fp32 state (h, e), caller's edge order, as numpy; t one timestep, or
+  one per edge (TSP) or node (MIS) in the caller's order."""
   V, ei, *_ = _case(case)
   row, col = torch.as_tensor(ei[0]), torch.as_tensor(ei[1])
   out = []
   for dt in (torch.float64, torch.float32):
     W = _weights(weights, dt)
-    temb = orc._time_emb(W, torch.tensor([T_LAYER], dtype=torch.float32))
+    temb = orc._time_emb(W, torch.as_tensor(np.asarray(t, np.float32)))
     hh, ee = orc.layer_step(W, layer, torch.as_tensor(h).to(dt), torch.as_tensor(e).to(dt), row, col, temb,
                             task == "tsp", agg)
     out.append((hh.numpy(), ee.numpy()))
@@ -192,22 +199,23 @@ TF_CASES = ([("tsp", "tsp"), ("tsp_shuf", "tsp"), ("mis", "mis"), ("dense50", "t
 _tf_cache = {}
 
 
-def _teacher_forced(weights, case, task, agg):
-  """Per layer l: the fp64 forward's state entering l rounded to fp32, and the fp64 / fp32 oracle layer l on it.  Only
-  the latest (case, task, agg) is kept: the parameters run in that order."""
-  key = (case, task, agg)
+def _teacher_forced(weights, case, task, agg, t=(T_LAYER,), t_key=None):
+  """Per layer l: the fp64 forward's state entering l rounded to fp32, and the fp64 / fp32 oracle layer l on it; t as
+  _refs, t_key names it.  Only the latest (case, task, agg, t_key) is kept: the parameters run in that order."""
+  key = (case, task, agg, t_key)
   if key not in _tf_cache:
     _tf_cache.clear()
     V, ei, *_ = _case(case)
     W = _weights(weights, torch.float64)
-    h, e, temb = _initial_state(W, task, case)
+    h, e, _ = _initial_state(W, task, case)
+    temb = orc._time_emb(W, torch.as_tensor(np.asarray(t, np.float32)))
     taps = []
     orc._sparse_encoding(W, h, e, torch.as_tensor(ei[0]), torch.as_tensor(ei[1]), temb, task == "tsp", agg, taps)
     states = [(h, e)] + taps[:-1]
     layers = []
     for l, (hs, es) in enumerate(states):
       h32, e32 = hs.numpy().astype(np.float32), es.numpy().astype(np.float32)
-      layers.append((h32, e32) + tuple(_refs(weights, task, case, l, h32, e32, agg)))
+      layers.append((h32, e32) + tuple(_refs(weights, task, case, l, h32, e32, agg, t)))
     _tf_cache[key] = layers
   return _tf_cache[key]
 

@@ -1,6 +1,6 @@
 """A timestep per element (the reference's training-step forwards), without a GPU: the fp32 oracle against the
-reference's outputs and losses in tests/golden/fwd_tsteps.npz, the Python timestep classification, and the code
-footprint of the edge kernel that reads a time vector per row."""
+reference's outputs and losses in tests/golden/fwd_tsteps.npz, the Python timestep classification, the code
+footprint of the edge kernel that reads a time vector per row, and the inputs of test_gpu_timesteps_edges.py."""
 import re
 
 import numpy as np
@@ -11,6 +11,8 @@ import torch.nn.functional as F
 from conftest import golden, rel_linf
 from oracle import difusco_oracle as orc
 from difusco_b200.models.gnn_encoder import MAX_TIMESTEPS, GNNEncoder, timestep_args
+import test_gpu_layer_parity as LP
+import test_gpu_timesteps_edges as TE
 import test_kernel_footprint as fp
 
 TOL = 1e-5   # fp32 restatement vs fp32 reference, as tests/test_oracle_golden.py
@@ -148,3 +150,78 @@ def test_trows_edge_kernel_registers_and_spills():
   assert m, "no resource usage for k_edge_layer_wg2_trows in the library"
   assert int(m.group(1)) == fp.REGS
   assert int(m.group(2)) <= fp.STACK_LIMIT, f"k_edge_layer_wg2_trows spill frame is {m.group(2)} bytes"
+
+
+# ---- the inputs of test_gpu_timesteps_edges.py are what they claim to be ----
+
+@pytest.mark.parametrize("case", TE.SHUF_TSP)
+def test_shuffled_graphs_are_unsorted(case):
+  """Every shuffled graph with two or more distinct rows reaches the kernels in an order the row sort changes, so
+  the lookup's perm branch runs (tiny1 and tiny2 have fewer edges than that can show)."""
+  V, ei, *_ = LP._case(case)
+  if len(np.unique(ei[0])) < 2:
+    pytest.skip(f"{case}: one distinct row")
+  assert (np.diff(ei[0]) < 0).any(), case
+  assert not np.array_equal(TE._sorted_perm(ei), np.arange(ei.shape[1]))
+
+
+@pytest.mark.parametrize("case", ["tsp_shuf", "hub_shuf", "degseq_shuf", "isolated_shuf", "dup_shuf", "tiny129_shuf"])
+def test_block_pattern_changes_exactly_at_warpgroup_and_tile_boundaries(case):
+  V, ei, *_ = LP._case(case)
+  t = TE.t_pattern(case, "tsp", "block")[TE._sorted_perm(ei)]   # sorted order
+  change = np.flatnonzero(np.diff(t) != 0) + 1                   # first sorted row of each new run
+  assert {64, 128} <= set(change.tolist()), case
+  assert (change % 64 == 0).all(), case
+  assert len(np.unique(t[:128])) == 2 and len(np.unique(t[:192])) == 3
+  values, index = TE.values_index(TE.t_pattern(case, "tsp", "block"))
+  assert np.array_equal(values[index], TE.t_pattern(case, "tsp", "block"))
+
+
+def test_nan_rows_are_the_boundary_rows_through_the_permutation():
+  V, ei, *_ = LP._case("hub_shuf")
+  rows = TE.nan_rows("hub_shuf", "tsp")
+  pos = np.argsort(TE._sorted_perm(ei))[rows]                    # sorted position of each chosen caller edge
+  assert sorted(pos.tolist()) == [0, 63, 64, 127, 128, ei.shape[1] - 1]
+  assert TE.nan_rows("mis", "mis").tolist() == [0, 63, 64, 127, 128, 149]
+
+
+def test_4096_timesteps_are_distinct_non_integers_in_fp32():
+  v = TE.max_t_values()
+  assert v.dtype == np.float32 and v.size == TE.MAX_T == MAX_TIMESTEPS
+  assert len(np.unique(v)) == v.size and (v != np.round(v)).all() and v.min() > 1 and v.max() < 1000
+  pts, ei, xt, index = TE._max_t_case()
+  assert ei.shape[1] >= TE.MAX_T and set(index.tolist()) == set(range(TE.MAX_T))
+  assert (np.diff(ei[0]) < 0).any()
+
+
+def test_oracle_per_row_layer_step_at_one_t_is_the_single_t_call(weights2):
+  V, ei, *_ = LP._case("tsp_shuf")
+  W = orc.Weights(weights2, torch.float64)
+  h, e, temb = LP._initial_state(W, "tsp", "tsp_shuf")
+  row, col = torch.as_tensor(ei[0]), torch.as_tensor(ei[1])
+  temb_rows = orc._time_emb(W, torch.full((ei.shape[1],), LP.T_LAYER, dtype=torch.float32))
+  for time_on_edge, rows in ((True, temb_rows), (False, temb_rows[:V])):
+    a = orc.layer_step(W, 3, h, e, row, col, temb, time_on_edge)
+    b = orc.layer_step(W, 3, h, e, row, col, rows, time_on_edge)
+    for x, y in zip(a, b):   # not bitwise: the time MLP runs as a GEMM on E rows and as a GEMV on one
+      assert float((x - y).abs().max() / y.abs().max()) < 1e-14
+
+
+def test_oracle_per_element_forward_is_invariant_to_edge_order(weights2):
+  """So one oracle run on the sorted graph serves the shuffled one (test_gpu_timesteps_edges.py)."""
+  pts, ei = TE.syn.tsp_sparse_batch(50, 20, 2, seed=5)
+  rng = np.random.default_rng(6)
+  t = rng.integers(1, 1001, ei.shape[1]).astype(np.float32)
+  xt = (rng.random(ei.shape[1]) < 0.3).astype(np.float32)
+  W = orc.Weights(weights2, torch.float64)
+  ref = orc.encoder_forward_sparse_tsp(W, pts, xt, t, ei).numpy()
+  eis, q = TE._shuffle(ei, 7)
+  got = TE._unshuffle(orc.encoder_forward_sparse_tsp(W, pts, xt[q], t[q], eis).numpy(), q)
+  assert rel_linf(got, ref) < 1e-12
+  V = 150
+  eim = TE.syn.er_graph_edge_index(V, 0.05, seed=8)
+  tv = rng.integers(1, 1001, V).astype(np.float32)
+  xv = (rng.random(V) < 0.5).astype(np.float32)
+  refm = orc.encoder_forward_mis(W, xv, tv, eim).numpy()
+  eims, _ = TE._shuffle(eim, 9)
+  assert rel_linf(orc.encoder_forward_mis(W, xv, tv, eims).numpy(), refm) < 1e-12

@@ -56,7 +56,7 @@ struct dfb_ctx {
   DevBuf d_row, d_col, d_perm, d_rowptr, d_grp_first, d_grp_pair, d_ei_stage, d_seg_start, d_seg_blk_first, d_gn_blk, d_local;
   // ---- workspace ----
   DevBuf e, h, h0, uvab, uvab0, partials, feat, tvec, gn_part, gn_stats, d_points, d_xt, d_u;
-  DevBuf opt_points, opt_tours, opt_pos, opt_dnext, opt_cand, opt_tiles, opt_state, opt_best, opt_inst, opt_tour_inst;   // 2-opt (row f3)
+  DevBuf opt_points, opt_tours, opt_pos, opt_dnext, opt_cand, opt_best, opt_table;   // 2-opt (row f3)
   // ---- step staging (pinned) + captured loop ----
   // dfb_denoise_step / dfb_denoise never allocate, never synchronise the host with the stream and never touch the
   // heap after the first call of a shape: timesteps and per-step parameters go through two pinned staging slots
@@ -1372,122 +1372,33 @@ extern "C" int dfb_tsp_merge_order(int64_t n, const int64_t* order, int64_t coun
   return r < 0 ? DFB_E_INVALID : r;
 }
 
-extern "C" int dfb_two_opt(dfb_ctx* ctx, const double* points, int64_t n, int64_t* tours, int64_t batch, int64_t max_iterations,
-                           int64_t* iterations_out, void* stream_) {
-  if (!ctx) return DFB_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream_;
-  CK(ctx, cudaSetDevice(ctx->device));
-  if (!points || !tours || !iterations_out) FAIL(ctx, DFB_E_INVALID, "two_opt: null argument");
-  if (n < 3 || n > 46340 || batch < 1 || batch > 65535) FAIL(ctx, DFB_E_INVALID, "two_opt: bad size n=%lld batch=%lld (n in [3, 46340], batch in [1, 65535])", (long long)n, (long long)batch);
-  const int N = (int)n, B = (int)batch;
-  bool finite = true;
-  for (int64_t k = 0; k < batch * (n + 1); ++k) {
-    if (tours[k] < 0 || tours[k] >= n) FAIL(ctx, DFB_E_INVALID, "two_opt: tour entry %lld out of range", (long long)tours[k]);
-    finite = finite && std::isfinite(points[2 * tours[k]]) && std::isfinite(points[2 * tours[k] + 1]);
-  }
-  if (!finite) {
-    // A NaN or inf point on a tour makes some move's change NaN; the reference's torch.min propagates it, its
-    // `min_change < -1e-6` test fails and it returns the tours unchanged after 0 iterations.
-    *iterations_out = 0;
-    return DFB_OK;
-  }
-  const int T = (N + TWOOPT_TILE - 1) / TWOOPT_TILE;
-  std::vector<int2> tiles;
-  for (int a = 0; a < T; ++a)
-    for (int b = a; b < T; ++b) tiles.push_back(make_int2(a, b));
-  const int ntiles = (int)tiles.size();
-  ENS(ctx, ctx->opt_points, (size_t)N * 2 * sizeof(double));
-  ENS(ctx, ctx->opt_tours, (size_t)B * (N + 1) * sizeof(long long));
-  ENS(ctx, ctx->opt_pos, (size_t)B * (N + 1) * 2 * sizeof(double));
-  ENS(ctx, ctx->opt_dnext, (size_t)B * N * sizeof(double));
-  ENS(ctx, ctx->opt_cand, (size_t)B * ntiles * sizeof(TwoOptCand));
-  ENS(ctx, ctx->opt_tiles, (size_t)ntiles * sizeof(int2));
-  ENS(ctx, ctx->opt_state, sizeof(TwoOptState));
-  ENS(ctx, ctx->opt_best, (size_t)B * sizeof(TwoOptCand));
-  double* d_points = (double*)ctx->opt_points.p;
-  long long* d_tours = (long long*)ctx->opt_tours.p;
-  double* d_pos = (double*)ctx->opt_pos.p;
-  double* d_dnext = (double*)ctx->opt_dnext.p;
-  TwoOptCand* d_cand = (TwoOptCand*)ctx->opt_cand.p;
-  int2* d_tiles = (int2*)ctx->opt_tiles.p;
-  TwoOptState* d_state = (TwoOptState*)ctx->opt_state.p;
-  CK(ctx, cudaMemcpyAsync(d_points, points, (size_t)N * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
-  CK(ctx, cudaMemcpyAsync(d_tours, tours, (size_t)B * (N + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
-  CK(ctx, cudaMemcpyAsync(d_tiles, tiles.data(), (size_t)ntiles * sizeof(int2), cudaMemcpyHostToDevice, st));
-  CK(ctx, cudaMemsetAsync(d_state, 0, sizeof(TwoOptState), st));
-  k_twoopt_init<<<dim3((N + 256) / 256, B), 256, 0, st>>>(d_points, d_tours, d_pos, d_dnext, N);
-  CKL(ctx);
-  TwoOptState hs{};
-  int chunk = 8;
-  while (true) {
-    for (int c = 0; c < chunk; ++c) {
-      k_twoopt_eval<<<dim3(ntiles, B), 256, 0, st>>>(d_pos, d_dnext, d_tiles, d_cand, d_state, N, ntiles);
-      CKL(ctx);
-      k_twoopt_apply<<<1, 1024, 0, st>>>(d_tours, d_pos, d_dnext, d_cand, d_state, (TwoOptCand*)ctx->opt_best.p, N, B, ntiles,
-                                         (long long)max_iterations);
-      CKL(ctx);
-    }
-    CK(ctx, cudaMemcpyAsync(&hs, d_state, sizeof(hs), cudaMemcpyDeviceToHost, st));
-    CK(ctx, cudaStreamSynchronize(st));
-    if (hs.done) break;
-    if (chunk < 64) chunk *= 2;
-  }
-  CK(ctx, cudaMemcpyAsync(tours, d_tours, (size_t)B * (N + 1) * sizeof(long long), cudaMemcpyDeviceToHost, st));
-  CK(ctx, cudaStreamSynchronize(st));
-  *iterations_out = hs.iterations;
-  return DFB_OK;
-}
-
-// dfb_two_opt over many instances at once: one work list of (instance, tour, tile) for the eval kernel, one apply block
-// per instance, every instance under its own stopping rule and cap.  Each instance's tours and iterations are those of
-// dfb_two_opt on it alone: the same tiles, candidates and reductions from per-instance base offsets.
-extern "C" int dfb_two_opt_instances(dfb_ctx* ctx, const double* points, const int64_t* node_ptr, int64_t n_instances,
-                                     const int64_t* tour_ptr, int64_t* tours, int64_t max_iterations,
-                                     int64_t* iterations_out, void* stream_) {
-  if (!ctx) return DFB_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream_;
-  CK(ctx, cudaSetDevice(ctx->device));
-  if (!points || !node_ptr || !tour_ptr || !tours || !iterations_out) FAIL(ctx, DFB_E_INVALID, "two_opt_instances: null argument");
-  if (n_instances < 1 || n_instances > 0x7fffffff)
-    FAIL(ctx, DFB_E_INVALID, "two_opt_instances: n_instances %lld out of range", (long long)n_instances);
-  if (node_ptr[0] != 0 || tour_ptr[0] != 0) FAIL(ctx, DFB_E_INVALID, "two_opt_instances: node_ptr and tour_ptr must start at 0");
-  const int NI = (int)n_instances;
+// The 2-opt of both entry points, on sizes they have checked: node_ptr and tour_ptr start at 0, every instance has n in
+// [3, 46340] and at least one tour, and the node and tour totals fit in int.  Checks the tour entries; one eval block
+// per (instance, tour, tile), one apply block per instance, every instance under its own stopping rule and cap, and
+// the host polls the count of running instances.
+static int two_opt_run(dfb_ctx* ctx, const double* points, const int64_t* node_ptr, int NI, const int64_t* tour_ptr,
+                       int64_t* tours, int64_t max_iterations, int64_t* iterations_out, cudaStream_t st) {
   std::vector<TwoOptInst> insts(NI);
-  std::vector<TwoOptState> states(NI);
   int64_t entries = 0, items = 0;
+  int running = 0, nmax = 0;
   for (int i = 0; i < NI; ++i) {
-    const int64_t n = node_ptr[i + 1] - node_ptr[i], B = tour_ptr[i + 1] - tour_ptr[i];
-    if (n < 3 || n > 46340) FAIL(ctx, DFB_E_INVALID, "two_opt_instances: instance %d has %lld nodes (must be in [3, 46340])", i, (long long)n);
-    if (B < 1) FAIL(ctx, DFB_E_INVALID, "two_opt_instances: instance %d has %lld tours (at least 1)", i, (long long)B);
-    if (node_ptr[i + 1] > 0x7fffffff || tour_ptr[i + 1] > 0x7fffffff)
-      FAIL(ctx, DFB_E_INVALID, "two_opt_instances: more than 2^31 - 1 nodes or tours");
-    const int T = (int)((n + TWOOPT_TILE - 1) / TWOOPT_TILE);
-    TwoOptInst& in = insts[i];
-    in.tour0 = entries;
-    in.dnext0 = entries - tour_ptr[i];
-    in.cand0 = items;
-    in.node0 = (int)node_ptr[i];
-    in.n = (int)n;
-    in.B = (int)B;
-    in.ntiles = T * (T + 1) / 2;
-    in.tour_first = (int)tour_ptr[i];
-    entries += B * (n + 1);
-    items += B * in.ntiles;
-    if (items > 0x7fffffff) FAIL(ctx, DFB_E_INVALID, "two_opt_instances: more than 2^31 - 1 eval tiles in one call");
-  }
-  int running = 0;
-  for (int i = 0; i < NI; ++i) {
-    const TwoOptInst& in = insts[i];
-    const double* p = points + 2 * (int64_t)in.node0;
+    const int n = (int)(node_ptr[i + 1] - node_ptr[i]), B = (int)(tour_ptr[i + 1] - tour_ptr[i]);
+    const int T = (n + TWOOPT_TILE - 1) / TWOOPT_TILE;
+    const double* p = points + 2 * node_ptr[i];
     bool finite = true;
-    for (int64_t k = in.tour0; k < in.tour0 + (int64_t)in.B * (in.n + 1); ++k) {
-      if (tours[k] < 0 || tours[k] >= in.n)
-        FAIL(ctx, DFB_E_INVALID, "two_opt_instances: instance %d: tour entry %lld out of range", i, (long long)tours[k]);
+    for (int64_t k = entries; k < entries + (int64_t)B * (n + 1); ++k) {
+      if (tours[k] < 0 || tours[k] >= n)
+        FAIL(ctx, DFB_E_INVALID, "two_opt: instance %d: tour entry %lld out of range", i, (long long)tours[k]);
       finite = finite && std::isfinite(p[2 * tours[k]]) && std::isfinite(p[2 * tours[k] + 1]);
     }
-    // as in dfb_two_opt: a non-finite point on a tour leaves the instance's tours unchanged after 0 iterations
-    states[i] = TwoOptState{finite ? 0 : 1, 0, 0};
+    // A NaN or inf point on a tour makes some move's change NaN; the reference's torch.min propagates it, its
+    // `min_change < -1e-6` test fails and it returns the tours unchanged after 0 iterations.
+    insts[i] = TwoOptInst{{finite ? 0 : 1, 0, 0}, entries, entries - tour_ptr[i], items, (int)node_ptr[i], n, B,
+                          T * (T + 1) / 2, (int)tour_ptr[i]};
     running += finite;
+    nmax = std::max(nmax, n);
+    entries += (int64_t)B * (n + 1);
+    items += (int64_t)B * insts[i].ntiles;
   }
   if (running == 0) {
     for (int i = 0; i < NI; ++i) iterations_out[i] = 0;
@@ -1495,54 +1406,40 @@ extern "C" int dfb_two_opt_instances(dfb_ctx* ctx, const double* points, const i
   }
   const int n_tours = (int)tour_ptr[NI];
   const int64_t V = node_ptr[NI];
-  std::vector<TwoOptWork> work((size_t)items);
-  std::vector<int> tour_inst(n_tours);
-  for (int i = 0; i < NI; ++i) {
-    const TwoOptInst& in = insts[i];
-    const int T = (in.n + TWOOPT_TILE - 1) / TWOOPT_TILE;
-    int64_t w = in.cand0;
-    for (int b = 0; b < in.B; ++b) {
-      tour_inst[in.tour_first + b] = i;
-      for (int a = 0; a < T; ++a)   // dfb_two_opt's tile order
-        for (int c = a; c < T; ++c) work[w++] = TwoOptWork{i, b, a, c};
-    }
-  }
+  // one upload of the per-call table: the instances with their states, then the running counter
+  const size_t inst_bytes = (size_t)NI * sizeof(TwoOptInst);
+  std::vector<char> table(inst_bytes + sizeof(int));
+  memcpy(table.data(), insts.data(), inst_bytes);
+  memcpy(table.data() + inst_bytes, &running, sizeof(int));
   ENS(ctx, ctx->opt_points, (size_t)V * 2 * sizeof(double));
   ENS(ctx, ctx->opt_tours, (size_t)entries * sizeof(long long));
   ENS(ctx, ctx->opt_pos, (size_t)entries * 2 * sizeof(double));
   ENS(ctx, ctx->opt_dnext, (size_t)(entries - n_tours) * sizeof(double));
   ENS(ctx, ctx->opt_cand, (size_t)items * sizeof(TwoOptCand));
-  ENS(ctx, ctx->opt_tiles, (size_t)items * sizeof(TwoOptWork));
-  ENS(ctx, ctx->opt_state, (size_t)NI * sizeof(TwoOptState) + sizeof(int));
   ENS(ctx, ctx->opt_best, (size_t)n_tours * sizeof(TwoOptCand));
-  ENS(ctx, ctx->opt_inst, (size_t)NI * sizeof(TwoOptInst));
-  ENS(ctx, ctx->opt_tour_inst, (size_t)n_tours * sizeof(int));
+  ENS(ctx, ctx->opt_table, table.size());
   double* d_points = (double*)ctx->opt_points.p;
   long long* d_tours = (long long*)ctx->opt_tours.p;
   double* d_pos = (double*)ctx->opt_pos.p;
   double* d_dnext = (double*)ctx->opt_dnext.p;
   TwoOptCand* d_cand = (TwoOptCand*)ctx->opt_cand.p;
-  TwoOptWork* d_work = (TwoOptWork*)ctx->opt_tiles.p;
-  TwoOptState* d_states = (TwoOptState*)ctx->opt_state.p;
-  int* d_running = (int*)(d_states + NI);
-  TwoOptInst* d_insts = (TwoOptInst*)ctx->opt_inst.p;
-  int* d_tour_inst = (int*)ctx->opt_tour_inst.p;
+  TwoOptInst* d_insts = (TwoOptInst*)ctx->opt_table.p;
+  int* d_running = (int*)(d_insts + NI);
   CK(ctx, cudaMemcpyAsync(d_points, points, (size_t)V * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
   CK(ctx, cudaMemcpyAsync(d_tours, tours, (size_t)entries * sizeof(long long), cudaMemcpyHostToDevice, st));
-  CK(ctx, cudaMemcpyAsync(d_work, work.data(), (size_t)items * sizeof(TwoOptWork), cudaMemcpyHostToDevice, st));
-  CK(ctx, cudaMemcpyAsync(d_states, states.data(), (size_t)NI * sizeof(TwoOptState), cudaMemcpyHostToDevice, st));
-  CK(ctx, cudaMemcpyAsync(d_running, &running, sizeof(int), cudaMemcpyHostToDevice, st));
-  CK(ctx, cudaMemcpyAsync(d_insts, insts.data(), (size_t)NI * sizeof(TwoOptInst), cudaMemcpyHostToDevice, st));
-  CK(ctx, cudaMemcpyAsync(d_tour_inst, tour_inst.data(), (size_t)n_tours * sizeof(int), cudaMemcpyHostToDevice, st));
-  k_twoopt_init_instances<<<n_tours, 256, 0, st>>>(d_points, d_tours, d_pos, d_dnext, d_insts, d_tour_inst);
+  CK(ctx, cudaMemcpyAsync(d_insts, table.data(), table.size(), cudaMemcpyHostToDevice, st));
+  k_twoopt_init<<<dim3(n_tours, (nmax + 256) / 256), 256, 0, st>>>(d_points, d_tours, d_pos, d_dnext, d_insts, NI);
   CKL(ctx);
   int chunk = 8;
   while (true) {
     for (int c = 0; c < chunk; ++c) {
-      k_twoopt_eval_instances<<<(unsigned)items, 256, 0, st>>>(d_pos, d_dnext, d_insts, d_work, d_cand, d_states);
-      CKL(ctx);
-      k_twoopt_apply_instances<<<NI, 1024, 0, st>>>(d_tours, d_pos, d_dnext, d_cand, d_insts, d_states,
-                                                     (TwoOptCand*)ctx->opt_best.p, d_running, (long long)max_iterations);
+      for (int64_t base = 0; base < items; base += 0x7fffffff) {   // a grid has at most 2^31 - 1 blocks
+        k_twoopt_eval<<<(unsigned)std::min<int64_t>(items - base, 0x7fffffff), 256, 0, st>>>(d_pos, d_dnext, d_insts, NI,
+                                                                                             d_cand, base);
+        CKL(ctx);
+      }
+      k_twoopt_apply<<<NI, 1024, 0, st>>>(d_tours, d_pos, d_dnext, d_cand, d_insts, (TwoOptCand*)ctx->opt_best.p, d_running,
+                                          (long long)max_iterations);
       CKL(ctx);
     }
     CK(ctx, cudaMemcpyAsync(&running, d_running, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1551,10 +1448,40 @@ extern "C" int dfb_two_opt_instances(dfb_ctx* ctx, const double* points, const i
     if (chunk < 64) chunk *= 2;
   }
   CK(ctx, cudaMemcpyAsync(tours, d_tours, (size_t)entries * sizeof(long long), cudaMemcpyDeviceToHost, st));
-  CK(ctx, cudaMemcpyAsync(states.data(), d_states, (size_t)NI * sizeof(TwoOptState), cudaMemcpyDeviceToHost, st));
+  CK(ctx, cudaMemcpyAsync(insts.data(), d_insts, inst_bytes, cudaMemcpyDeviceToHost, st));
   CK(ctx, cudaStreamSynchronize(st));
-  for (int i = 0; i < NI; ++i) iterations_out[i] = states[i].iterations;
+  for (int i = 0; i < NI; ++i) iterations_out[i] = insts[i].st.iterations;
   return DFB_OK;
+}
+
+extern "C" int dfb_two_opt(dfb_ctx* ctx, const double* points, int64_t n, int64_t* tours, int64_t batch, int64_t max_iterations,
+                           int64_t* iterations_out, void* stream_) {
+  if (!ctx) return DFB_E_INVALID;
+  CK(ctx, cudaSetDevice(ctx->device));
+  if (!points || !tours || !iterations_out) FAIL(ctx, DFB_E_INVALID, "two_opt: null argument");
+  if (n < 3 || n > 46340 || batch < 1 || batch > 65535) FAIL(ctx, DFB_E_INVALID, "two_opt: bad size n=%lld batch=%lld (n in [3, 46340], batch in [1, 65535])", (long long)n, (long long)batch);
+  const int64_t node_ptr[2] = {0, n}, tour_ptr[2] = {0, batch};
+  return two_opt_run(ctx, points, node_ptr, 1, tour_ptr, tours, max_iterations, iterations_out, (cudaStream_t)stream_);
+}
+
+extern "C" int dfb_two_opt_instances(dfb_ctx* ctx, const double* points, const int64_t* node_ptr, int64_t n_instances,
+                                     const int64_t* tour_ptr, int64_t* tours, int64_t max_iterations,
+                                     int64_t* iterations_out, void* stream_) {
+  if (!ctx) return DFB_E_INVALID;
+  CK(ctx, cudaSetDevice(ctx->device));
+  if (!points || !node_ptr || !tour_ptr || !tours || !iterations_out) FAIL(ctx, DFB_E_INVALID, "two_opt_instances: null argument");
+  if (n_instances < 1 || n_instances > 0x7fffffff)
+    FAIL(ctx, DFB_E_INVALID, "two_opt_instances: n_instances %lld out of range", (long long)n_instances);
+  if (node_ptr[0] != 0 || tour_ptr[0] != 0) FAIL(ctx, DFB_E_INVALID, "two_opt_instances: node_ptr and tour_ptr must start at 0");
+  for (int64_t i = 0; i < n_instances; ++i) {
+    const int64_t n = node_ptr[i + 1] - node_ptr[i], B = tour_ptr[i + 1] - tour_ptr[i];
+    if (n < 3 || n > 46340) FAIL(ctx, DFB_E_INVALID, "two_opt_instances: instance %lld has %lld nodes (must be in [3, 46340])", (long long)i, (long long)n);
+    if (B < 1) FAIL(ctx, DFB_E_INVALID, "two_opt_instances: instance %lld has %lld tours (at least 1)", (long long)i, (long long)B);
+    if (node_ptr[i + 1] > 0x7fffffff || tour_ptr[i + 1] > 0x7fffffff)
+      FAIL(ctx, DFB_E_INVALID, "two_opt_instances: more than 2^31 - 1 nodes or tours");
+  }
+  return two_opt_run(ctx, points, node_ptr, (int)n_instances, tour_ptr, tours, max_iterations, iterations_out,
+                     (cudaStream_t)stream_);
 }
 
 // Row f4: text heat map for tsp_mcts (convert_numpy_to_txt.py:57-73).  Most entries are exactly zero after the

@@ -237,21 +237,31 @@ __device__ __forceinline__ double twoopt_dist(double ax, double ay, double bx, d
   return __dsqrt_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)));
 }
 
-// Per instance of dfb_two_opt_instances: where its tours start in the concatenated buffers and its shape.  Its B tours of
-// n + 1 entries are consecutive, so from these bases on the instance is exactly one dfb_two_opt problem.
+// One instance of a 2-opt call: its state, where its tours start in the concatenated buffers and its shape.  Its B
+// tours of n + 1 entries are consecutive, and its eval items, one per tour and tile, run tour-major from cand0 on.
+// dfb_two_opt is the call with one instance.
 struct TwoOptInst {
+  TwoOptState st;     // written by k_twoopt_apply; read with the rest in one hop by k_twoopt_eval
   long long tour0;    // first entry of its first tour in tours (pos: 2 x)
   long long dnext0;   // first entry in dnext (n per tour)
-  long long cand0;    // first candidate slot (= first work item; ntiles per tour)
+  long long cand0;    // first eval item and candidate slot (ntiles per tour)
   int node0;          // first node in points
   int n, B, ntiles;
   int tour_first;     // global index of its first tour (slot in the per-tour arg-min array)
 };
-// One eval block of dfb_two_opt_instances: instance, its tour, and the tile (a, b).  The list is instance-major, then tour,
-// then tile, so an instance's candidates have dfb_two_opt's layout from TwoOptInst::cand0 on.
-struct TwoOptWork {
-  int inst, tour, a, b;
-};
+
+// The last instance whose first key (cand0 or tour_first; ascending) is <= x: a binary search, with no load for one
+// instance.
+template <typename K>
+__device__ __forceinline__ int twoopt_instance(const TwoOptInst* __restrict__ insts, int ni, K TwoOptInst::*first,
+                                               long long x) {
+  int i = 0;
+  for (int hi = ni; hi - i > 1;) {
+    const int mid = (i + hi) >> 1;
+    if (insts[mid].*first <= x) i = mid; else hi = mid;
+  }
+  return i;
+}
 
 // One tour's pos (N+1, 2) and dnext (N): coordinates along the tour and |pos[k] - pos[k+1]|.  Entries k0, k0 + stride, ...
 __device__ __forceinline__ void twoopt_init_tour(const double* __restrict__ points, const long long* __restrict__ tour,
@@ -267,23 +277,27 @@ __device__ __forceinline__ void twoopt_init_tour(const double* __restrict__ poin
   }
 }
 
-// pos (B, N+1, 2): coordinates along the tour; dnext (B, N): |pos[k] - pos[k+1]|.
-__global__ void k_twoopt_init(const double* __restrict__ points, const long long* __restrict__ tours, double* __restrict__ pos,
-                              double* __restrict__ dnext, int N) {
-  const int b = blockIdx.y;
-  twoopt_init_tour(points, tours + (size_t)b * (N + 1), pos + (size_t)b * (N + 1) * 2, dnext + (size_t)b * N, N,
-                   blockIdx.x * blockDim.x + threadIdx.x, gridDim.x * blockDim.x);
-}
-
-// One block per tour of every instance.
-__global__ void k_twoopt_init_instances(const double* __restrict__ points, const long long* __restrict__ tours,
-                                        double* __restrict__ pos, double* __restrict__ dnext,
-                                        const TwoOptInst* __restrict__ insts, const int* __restrict__ tour_inst) {
-  const TwoOptInst in = insts[tour_inst[blockIdx.x]];
-  const long long t = blockIdx.x - in.tour_first;
+// grid (every tour of every instance, chunks of blockDim.x entries of the longest tour)
+__global__ void k_twoopt_init(const double* __restrict__ points, const long long* __restrict__ tours,
+                              double* __restrict__ pos, double* __restrict__ dnext, const TwoOptInst* __restrict__ insts,
+                              int ni) {
+  const TwoOptInst in = insts[twoopt_instance(insts, ni, &TwoOptInst::tour_first, blockIdx.x)];
+  const long long t = (long long)blockIdx.x - in.tour_first;
   const long long e0 = in.tour0 + t * (in.n + 1);
   twoopt_init_tour(points + 2 * (size_t)in.node0, tours + e0, pos + 2 * e0, dnext + in.dnext0 + t * in.n, in.n,
-                   threadIdx.x, blockDim.x);
+                   blockIdx.y * blockDim.x + threadIdx.x, gridDim.y * blockDim.x);
+}
+
+// Tile k of the T x T upper triangle in a-major order (0,0) ... (0,T-1), (1,1), ...  Counted from the end, r is entry
+// p of row q of the reversed triangle, whose rows hold 1, 2, ... tiles: q is the largest with q(q+1)/2 <= r, the
+// floor of (sqrt(8r + 1) - 1) / 2.  A float estimate and one correction each way make it exact.
+__device__ __forceinline__ int2 twoopt_tile(int k, int T) {
+  const int r = T * (T + 1) / 2 - 1 - k;
+  const float x = (float)(8 * r + 1);
+  int q = (int)((x * rsqrtf(x) - 1.0f) * 0.5f);
+  q += (q + 1) * (q + 2) / 2 <= r;
+  q -= q * (q + 1) / 2 > r;
+  return make_int2(T - 1 - q, T - 1 - (r - q * (q + 1) / 2));
 }
 
 // The best move of one 64x64 tile (i in tile row t.x, j in tile column t.y, j >= i + 2) of one tour, by one block of 256
@@ -352,29 +366,29 @@ __device__ __forceinline__ void twoopt_eval_tile(const double* __restrict__ P, c
   }
 }
 
-// grid (tiles, B)
+// One block per eval item base + blockIdx.x: its instance, tour and tile; the candidate goes to slot item.  The blocks
+// of a finished instance return at once.  Thread 0 alone works out the block's tour and tile: in every thread that
+// arithmetic costs a measurable share of the tile's own.
 __global__ void __launch_bounds__(256) k_twoopt_eval(const double* __restrict__ pos, const double* __restrict__ dnext,
-                                                     const int2* __restrict__ tiles, TwoOptCand* __restrict__ cand,
-                                                     const TwoOptState* __restrict__ state, int N, int ntiles) {
-  if (state->done) return;
-  const int b = blockIdx.y;
-  twoopt_eval_tile(pos + (size_t)b * (N + 1) * 2, dnext + (size_t)b * N, tiles[blockIdx.x], N,
-                   cand + (size_t)b * ntiles + blockIdx.x);
-}
-
-// One block per work item of every instance; the blocks of a finished instance return at once.
-__global__ void __launch_bounds__(256) k_twoopt_eval_instances(const double* __restrict__ pos,
-                                                               const double* __restrict__ dnext,
-                                                               const TwoOptInst* __restrict__ insts,
-                                                               const TwoOptWork* __restrict__ work,
-                                                               TwoOptCand* __restrict__ cand,
-                                                               const TwoOptState* __restrict__ states) {
-  const TwoOptWork w = work[blockIdx.x];
-  if (states[w.inst].done) return;
-  const TwoOptInst in = insts[w.inst];
-  const long long e0 = in.tour0 + (long long)w.tour * (in.n + 1);
-  twoopt_eval_tile(pos + 2 * e0, dnext + in.dnext0 + (long long)w.tour * in.n, make_int2(w.a, w.b), in.n,
-                   cand + blockIdx.x);
+                                                     const TwoOptInst* __restrict__ insts, int ni,
+                                                     TwoOptCand* __restrict__ cand, long long base) {
+  __shared__ long long s_p0, s_d0;
+  __shared__ int2 s_tile;
+  __shared__ int s_n;   // 0: the instance is done
+  const long long item = base + blockIdx.x;
+  if (threadIdx.x == 0) {
+    const TwoOptInst in = insts[twoopt_instance(insts, ni, &TwoOptInst::cand0, item)];
+    s_n = in.st.done ? 0 : in.n;
+    if (!in.st.done) {
+      const long long t = (item - in.cand0) / in.ntiles;
+      s_p0 = 2 * (in.tour0 + t * (in.n + 1));
+      s_d0 = in.dnext0 + t * in.n;
+      s_tile = twoopt_tile((int)(item - in.cand0 - t * in.ntiles), (in.n + TWOOPT_TILE - 1) / TWOOPT_TILE);
+    }
+  }
+  __syncthreads();
+  if (s_n == 0) return;
+  twoopt_eval_tile(pos + s_p0, dnext + s_d0, s_tile, s_n, cand + item);
 }
 
 // One iteration of one batch of B tours, by one block of 1024 threads: reduce the tile candidates of every tour, take the
@@ -457,27 +471,15 @@ __device__ __forceinline__ void twoopt_apply_batch(long long* __restrict__ tours
   }
 }
 
-// Single block: one iteration of dfb_two_opt's batch.
-__global__ void __launch_bounds__(1024) k_twoopt_apply(long long* __restrict__ tours, double* __restrict__ pos,
-                                                       double* __restrict__ dnext, const TwoOptCand* __restrict__ cand,
-                                                       TwoOptState* __restrict__ state, TwoOptCand* __restrict__ s_best,
-                                                       int N, int B, int ntiles, long long max_iterations) {
-  twoopt_apply_batch(tours, pos, dnext, cand, state, s_best, N, B, ntiles, max_iterations);
-}
-
 // One block per instance: one iteration of its own batch, under its own stopping rule and cap.  An instance that stops
 // takes itself off *running, the counter the host polls.
-__global__ void __launch_bounds__(1024) k_twoopt_apply_instances(long long* __restrict__ tours, double* __restrict__ pos,
-                                                                 double* __restrict__ dnext,
-                                                                 const TwoOptCand* __restrict__ cand,
-                                                                 const TwoOptInst* __restrict__ insts,
-                                                                 TwoOptState* __restrict__ states,
-                                                                 TwoOptCand* __restrict__ s_best, int* __restrict__ running,
-                                                                 long long max_iterations) {
-  TwoOptState* st = states + blockIdx.x;
-  if (st->done) return;
-  const TwoOptInst in = insts[blockIdx.x];
-  twoopt_apply_batch(tours + in.tour0, pos + 2 * in.tour0, dnext + in.dnext0, cand + in.cand0, st, s_best + in.tour_first,
-                     in.n, in.B, in.ntiles, max_iterations);
-  if (threadIdx.x == 0 && st->done) atomicSub(running, 1);   // thread 0 is the one that sets done
+__global__ void __launch_bounds__(1024) k_twoopt_apply(long long* __restrict__ tours, double* __restrict__ pos,
+                                                       double* __restrict__ dnext, const TwoOptCand* __restrict__ cand,
+                                                       TwoOptInst* __restrict__ insts, TwoOptCand* __restrict__ s_best,
+                                                       int* __restrict__ running, long long max_iterations) {
+  TwoOptInst* in = insts + blockIdx.x;
+  if (in->st.done) return;
+  twoopt_apply_batch(tours + in->tour0, pos + 2 * in->tour0, dnext + in->dnext0, cand + in->cand0, &in->st,
+                     s_best + in->tour_first, in->n, in->B, in->ntiles, max_iterations);
+  if (threadIdx.x == 0 && in->st.done) atomicSub(running, 1);   // thread 0 is the one that sets done
 }

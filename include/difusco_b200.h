@@ -217,17 +217,20 @@ int dfb_tsp_merge_order(int64_t n, const int64_t* order, int64_t count, int64_t*
 
 /* Row f3: batched 2-opt, utils/tsp_utils.py:12-49 (batched_two_opt_torch).  points (n,2) float64 HOST, tours
  * (batch, n+1) int64 HOST, updated in place; iterations_out = the reference's `iterator`.  Same moves in the same
- * order as the reference on its CPU device (float64, first-occurrence arg-min, batch-wide stopping rule). */
+ * order as the reference on its CPU device (float64, first-occurrence arg-min, batch-wide stopping rule).  The
+ * one-instance case of dfb_two_opt_instances (node_ptr = {0, n}, tour_ptr = {0, batch}), with n in [3, 46340] and
+ * batch in [1, 65535]; DFB_E_INVALID, tours untouched, otherwise. */
 int dfb_two_opt(dfb_ctx* ctx, const double* points, int64_t n, int64_t* tours, int64_t batch, int64_t max_iterations,
                 int64_t* iterations_out, void* stream);
 
-/* dfb_two_opt over many instances in one call.  points (V,2) float64 HOST; instance i owns nodes
+/* 2-opt over many instances in one call.  points (V,2) float64 HOST; instance i owns nodes
  * [node_ptr[i], node_ptr[i+1]) and tours [tour_ptr[i], tour_ptr[i+1]) (both HOST, n_instances + 1 entries, starting at
  * 0); tours HOST, the instances' rows of n_i + 1 LOCAL node ids concatenated, updated in place; iterations_out HOST
- * (n_instances,).  Every instance's tours and iteration count are exactly dfb_two_opt's on that instance alone: the
- * same moves and float64 arithmetic, its own batch-wide stopping rule and its own cap; an instance with a non-finite
- * point on a tour is returned unchanged after 0 iterations while the others run.  n_i in [3, 46340], at least one
- * tour per instance, no limit on the tour count of one instance; DFB_E_INVALID, tours untouched, otherwise. */
+ * (n_instances,).  Every instance's tours and iteration count are those it gets alone: the same moves and float64
+ * arithmetic, its own batch-wide stopping rule and its own cap; an instance with a non-finite point on a tour is
+ * returned unchanged after 0 iterations while the others run.  n_i in [3, 46340], at least one tour per instance, at
+ * most 2^31 - 1 nodes and 2^31 - 1 tours in all, no limit on the tour count of one instance or on the number of
+ * (tour, 64 x 64 tile) pairs of a call; DFB_E_INVALID, tours untouched, otherwise. */
 int dfb_two_opt_instances(dfb_ctx* ctx, const double* points, const int64_t* node_ptr, int64_t n_instances,
                           const int64_t* tour_ptr, int64_t* tours, int64_t max_iterations, int64_t* iterations_out,
                           void* stream);

@@ -18,7 +18,8 @@
 // Two consumer warpgroups take turns on the tensor cores (ping-pong): one runs a GEMM alone while the other runs an
 // epilogue, so each GEMM overlaps the other warpgroup's memory waits instead of sharing the tensor cores with its GEMM.
 // Per-(32-edge group, node) message sums go through shared memory (the dead GEMM1 operand) and are reduced in a fixed
-// order per column: deterministic, no atomics.
+// order per column: deterministic, no atomics.  The whole rows the epilogues read (V h[col] in E1, e_in in E4) are
+// copied into the dead operand area with cp.async once a GEMM has drained, so they wait on memory without registers.
 // Precision: every 256x256 product is evaluated as  a_hi*b_hi + a_lo*b_hi + a_hi*b_lo  with
 // a = a_hi + a_lo, b = b_hi + b_lo in bf16 and fp32 accumulation: ~2^-17 relative error per product, which keeps the
 // 1e-4 fp32 contract (single-pass TF32/BF16 does not: SURVEY D9).
@@ -42,10 +43,9 @@ constexpr int TC_KCH = 64;                      // K elements per chunk = one 12
 constexpr int TC_B_BYTES = 256 * 128;           // one weight chunk [256 rows x 64 K] bf16 (hi or lo)
 constexpr int TC_A_CHUNK = WG_ROWS * 128;       // one operand chunk [64 rows x 64 K] bf16 (hi or lo)
 constexpr int TC_A_BYTES = 8 * TC_A_CHUNK;      // 4 K-chunks x (hi, lo) per warpgroup = 64 KB = [64][256] fp32 messages
-// Loads a consumer thread issues before it uses the first of them (memory-level parallelism of the epilogues), sized
-// so that they fit next to the 128 accumulator registers without spills:
-constexpr int CONV_BATCH = 16;   // conversion: float4 row loads of 32
-constexpr int E4_BATCH = 16;     // E4: float2 e_in loads of a row half of 32
+// Row loads a consumer thread issues in the conversion before it uses the first of them (memory-level parallelism),
+// sized so that they fit next to the 128 accumulator registers without spills: float4 row loads of 32
+constexpr int CONV_BATCH = 16;
 
 // The bf16 weight arena, the tensor-core kernels' B operand: every row offset into it comes from here.
 // Each 256x256 matrix W [out][in] takes two blocks of 256 rows, K-major: hi = bf16(W), then lo = bf16(W - hi).
@@ -152,6 +152,13 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// 16-byte global -> shared copy through L2 only; it holds no register while in flight
+__device__ __forceinline__ void cp_async16(void* dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// the thread's own copies have landed; a __syncwarp after it shows them to the rest of the warp
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
 // K-major, 128-byte swizzle, 8-row atoms 1024 bytes apart (wgmma shared-memory matrix descriptor)
 __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
@@ -228,6 +235,9 @@ __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t&
 __device__ __forceinline__ uint32_t sw128_off(int r, int j) {
   return (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((j ^ (r & 7)) << 4));
 }
+// (c ^ 8 (r & 7)) - c % 8 for the column pair c = 8 j + 2 t of row r in the message layout.  Written so that the 32 pairs
+// of a row share 8 XORs and differ by immediate offsets (j is a compile-time constant).
+__device__ __forceinline__ int msg_col(int j, int r) { return 64 * (j >> 3) + ((8 * (j & 7)) ^ (8 * (r & 7))); }
 __device__ __forceinline__ float quad_sum(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 1);
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
@@ -435,6 +445,22 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
     }
   };
 
+  // Copies the 1 KB rows row_src(i), i < 16, into this warp's rows 16 wi + i of the dead operand area, in the message
+  // layout, with cp.async: a whole tile's rows are in flight at once without holding a register.  Each lane copies the
+  // same two 16-byte column groups of every row, which the XOR swizzle keeps intact.  Only valid after a GEMM has
+  // drained (wait_group 0: no wgmma reads the area any more).  Waited on with cp_async_wait_all and a __syncwarp.
+  auto stage_rows = [&](auto row_src) {
+#pragma unroll 1
+    for (int i = 0; i < 16; ++i) {
+      const int r = wi * 16 + i;
+      const float* src = row_src(i) + 4 * lane;
+      float* dst = msg + r * H + ((4 * lane) ^ (8 * (r & 7)));
+      cp_async16(dst, src);
+      cp_async16(dst + 128, src + 128);
+    }
+    cp_async_commit();
+  };
+
   for (int tile = blockIdx.x; tile < P.n_tiles; tile += gridDim.x) {
     record(PH_TILES, 1);
     const int row_tile = (lin && P.lin_nb == 4) ? (tile >> 2) : tile;
@@ -510,27 +536,36 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
 
     // ---------------- E1: e_hat = acc + A h[col] + B h[row];  messages sigmoid(e_hat) * V h[col] ----------------
     // E1 and E2 / E3 run once per row half h (rows lr0, lr0 + 8) on acc[4 j], acc[4 j + 1], then swap the halves.
-    const float* src_a = w_src[lr0];
-    const float* src_b = w_src[lr0 + 8];
+    // V h[col] of the warp's 16 rows is copied to where the rows' messages go.  Each pass gathers A h[col] and B h[row]
+    // into the accumulator, then turns each V value into its message in place.  Lane i (and i + 16) holds row i's col.
+    const int s_lane = s_base + wi * 16 + (lane & 15);
+    const int col_lane = s_lane < n_rows ? P.g.col[s_lane] : 0;
+    stage_rows([&](int i) { return P.uvab + (size_t)__shfl_sync(0xffffffffu, col_lane, i) * 4 * H + H; });
 #pragma unroll 1
     for (int h = 0; h < 2; ++h) {
-      const int s = h ? sb : sa;
       const bool v = h ? vb : va;
-      const float* cp = P.uvab + (size_t)(v ? P.g.col[s] : 0) * 4 * H;
-      const float* rp = P.uvab + (size_t)(v ? P.g.row[s] : 0) * 4 * H + 3 * H;
-      const int r = lr0 + 8 * h;
+      const float* ap = P.uvab + (size_t)__shfl_sync(0xffffffffu, col_lane, (lane >> 2) + 8 * h) * 4 * H + 2 * H;
+      const float* bp = P.uvab + (size_t)(v ? P.g.row[h ? sb : sa] : 0) * 4 * H + 3 * H;
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         const int c = 8 * j + 2 * t4;
-        const float2 ah = __ldg(reinterpret_cast<const float2*>(cp + 2 * H + c));
-        const float2 vh = __ldg(reinterpret_cast<const float2*>(cp + H + c));
-        const float2 bh = __ldg(reinterpret_cast<const float2*>(rp + c));
-        const float x0 = (acc[4 * j] + ah.x) + bh.x;
-        const float x1 = (acc[4 * j + 1] + ah.y) + bh.y;
-        acc[4 * j] = x0;
-        acc[4 * j + 1] = x1;
-        *reinterpret_cast<float2*>(msg + r * H + (c ^ (8 * (r & 7)))) =
-            make_float2(sigmoid_mufu(x0) * vh.x, sigmoid_mufu(x1) * vh.y);
+        const float2 ah = __ldg(reinterpret_cast<const float2*>(ap + c));
+        const float2 bh = __ldg(reinterpret_cast<const float2*>(bp + c));
+        acc[4 * j] = (acc[4 * j] + ah.x) + bh.x;
+        acc[4 * j + 1] = (acc[4 * j + 1] + ah.y) + bh.y;
+      }
+      // The copies are waited for once, after the first pass's gathers.  As a block of its own the wait stays behind
+      // them; inside the loop body's block ptxas scheduled it ahead of every gather.
+      if (h == 0) {
+        cp_async_wait_all();
+        __syncwarp();
+      }
+      float* m = msg + (lr0 + 8 * h) * H + 2 * t4;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        float2* mp = reinterpret_cast<float2*>(m + msg_col(j, lr0));
+        const float2 vh = *mp;
+        *mp = make_float2(sigmoid_mufu(acc[4 * j]) * vh.x, sigmoid_mufu(acc[4 * j + 1]) * vh.y);
       }
       swap_row_halves(acc);
     }
@@ -628,33 +663,36 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
       }
       swap_row_halves(acc);
     }
+    // E4's e_in rows (lane i and i + 16 hold row i's), read before the barrier: a warp past it may go on to the next
+    // tile and rewrite the row table
+    const float* e_src = w_src[wi * 16 + (lane & 15)];
     fence_proxy_async();
     wg_bar();
     mark(PH_LN);
     gemm(PH_G2_WAIT, PH_G2_MMA);   // GEMM2: acc = s * O^T
 
     // ---------------- E4: e = e_in + O(s) + b_O (in place) ----------------
-    // Both row halves stay unrolled here: as a rolled loop over h (swapping or shifting the halves), ptxas fails to
-    // allocate registers for the kernel at 232 per thread.
+    // The warp's e_in rows are staged in the operand area and have all landed before the first store to a row, so the
+    // in-place update needs no ordering of its own.  Both row halves stay unrolled here: as a rolled loop over h
+    // (swapping or shifting the halves), ptxas fails to allocate registers for the kernel at 232 per thread.
+    stage_rows([&](int i) {
+      return reinterpret_cast<const float*>(__shfl_sync(0xffffffffu, reinterpret_cast<unsigned long long>(e_src), i));
+    });
+    cp_async_wait_all();
+    __syncwarp();
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       if (!(h ? vb : va)) continue;
-      const float* src = h ? src_b : src_a;
+      const int r = lr0 + 8 * h;
+      const float* er = msg + r * H + 2 * t4;
       float* dst = P.e + (size_t)(h ? sb : sa) * H;
-      // the row is updated in place: its e_in values are loaded in batches before any of them is overwritten (the
-      // compiler cannot move a load above a store to the same row by itself)
 #pragma unroll
-      for (int j0 = 0; j0 < 32; j0 += E4_BATCH) {
-        float2 ein[E4_BATCH];
-#pragma unroll
-        for (int q = 0; q < E4_BATCH; ++q) ein[q] = __ldcg(reinterpret_cast<const float2*>(src + 8 * (j0 + q) + 2 * t4));
-#pragma unroll
-        for (int q = 0; q < E4_BATCH; ++q) {
-          const int j = j0 + q, c = 8 * j + 2 * t4;
-          const float2 bo = *reinterpret_cast<const float2*>(prm + 5 * H + c);
-          __stcg(reinterpret_cast<float2*>(dst + c),
-                 make_float2((ein[q].x + acc[4 * j + 2 * h]) + bo.x, (ein[q].y + acc[4 * j + 2 * h + 1]) + bo.y));
-        }
+      for (int j = 0; j < 32; ++j) {
+        const int c = 8 * j + 2 * t4;
+        const float2 ein = *reinterpret_cast<const float2*>(er + msg_col(j, r));
+        const float2 bo = *reinterpret_cast<const float2*>(prm + 5 * H + c);
+        __stcg(reinterpret_cast<float2*>(dst + c),
+               make_float2((ein.x + acc[4 * j + 2 * h]) + bo.x, (ein.y + acc[4 * j + 2 * h + 1]) + bo.y));
       }
     }
     mark(PH_E4);

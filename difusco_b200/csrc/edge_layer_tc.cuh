@@ -11,10 +11,10 @@
 //                         converts its fp32 rows into the bf16 hi/lo A operand, runs GEMM1, the gate / message /
 //                         LayerNorm epilogues straight out of the accumulator registers (a row lives in the 4 threads
 //                         of a quad), writes GEMM2's A operand over GEMM1's and finishes with the residual update.
-//   warpgroup NWG         TMA producer (one thread): streams the bf16 hi/lo weight K-chunks [256 rows x 64 K] (128B
-//                         swizzle) through an NSTAGE ring, each GEMM's 8 chunks once per consumer warpgroup.  With two
-//                         consumer warpgroups it hands its registers to them (setmaxnreg 40 / 232): no spills in the
-//                         epilogue.
+//   warpgroup NWG         TMA producer (one thread): streams the bf16 hi/lo weight K-chunks [256 rows x 32 K] (16 KB,
+//                         64B swizzle) through a 4-stage ring, each GEMM's 16 chunks once per consumer warpgroup, so
+//                         three chunks are in flight while the tensor cores read the fourth.  With two consumer
+//                         warpgroups it hands its registers to them (setmaxnreg 40 / 232): no spills in the epilogue.
 // Two consumer warpgroups take turns on the tensor cores (ping-pong): one runs a GEMM alone while the other runs an
 // epilogue, so each GEMM overlaps the other warpgroup's memory waits instead of sharing the tensor cores with its GEMM.
 // Per-(32-edge group, node) message sums go through shared memory (the dead GEMM1 operand) and are reduced in a fixed
@@ -39,8 +39,10 @@
 namespace dfb {
 
 constexpr int WG_ROWS = 64;                     // rows per consumer warpgroup (wgmma M)
-constexpr int TC_KCH = 64;                      // K elements per chunk = one 128-byte swizzle row of bf16
-constexpr int TC_B_BYTES = 256 * 128;           // one weight chunk [256 rows x 64 K] bf16 (hi or lo)
+constexpr int TC_KBLK = 64;                     // K elements per A-operand chunk = one 128-byte swizzle row of bf16
+constexpr int TC_KCH = 32;                      // K elements per weight chunk = one 64-byte swizzle row of bf16
+constexpr int TC_B_BYTES = 256 * TC_KCH * 2;    // one weight chunk [256 rows x 32 K] bf16 (hi or lo) = 16 KB
+static_assert(TC_KCH * 2 == 64, "weight chunk rows are one 64-byte swizzle row (tensor map, wgmma_desc_sw64)");
 constexpr int TC_A_CHUNK = WG_ROWS * 128;       // one operand chunk [64 rows x 64 K] bf16 (hi or lo)
 constexpr int TC_A_BYTES = 8 * TC_A_CHUNK;      // 4 K-chunks x (hi, lo) per warpgroup = 64 KB = [64][256] fp32 messages
 // Row loads a consumer thread issues in the conversion before it uses the first of them (memory-level parallelism),
@@ -65,7 +67,8 @@ struct TcCfg {
   static_assert(NWG == 1 || NWG == 2, "one or two consumer warpgroups");
   static constexpr int TILE = NWG * WG_ROWS;
   static constexpr int THREADS = (NWG + 1) * 128;
-  static constexpr int NSTAGE = (NWG == 1) ? 3 : 2;
+  // one stage per weight chunk of a K block: hi K[0,32), hi K[32,64), lo K[0,32), lo K[32,64)
+  static constexpr int NSTAGE = 2 * TC_KBLK / TC_KCH;
   static constexpr int OFF_B = NWG * TC_A_BYTES;
   static constexpr int OFF_PRM = OFF_B + NSTAGE * TC_B_BYTES;   // ln_e_g, ln_e_b, tau, ln_o_g, ln_o_b, b_O
   static constexpr int OFF_ROW = OFF_PRM + 6 * H * 4;
@@ -160,9 +163,13 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 // the thread's own copies have landed; a __syncwarp after it shows them to the rest of the warp
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
-// K-major, 128-byte swizzle, 8-row atoms 1024 bytes apart (wgmma shared-memory matrix descriptor)
+// K-major, 128-byte swizzle, 8-row atoms 1024 bytes apart (wgmma shared-memory matrix descriptor): the A operand
 __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
   return (uint64_t)((smem_addr >> 4) & 0x3fffu) | (1ull << 16) | (64ull << 32) | (1ull << 62);
+}
+// K-major, 64-byte swizzle, 8-row atoms 512 bytes apart: the weight chunks (the k16 steps of a row are 32 bytes apart)
+__device__ __forceinline__ uint64_t wgmma_desc_sw64(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr >> 4) & 0x3fffu) | (1ull << 16) | (32ull << 32) | (2ull << 62);
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -303,8 +310,8 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr bool lin = LIN;
-  // (C | O) x consumer warpgroup x 4 K-chunks x (hi, lo): C for warpgroup 0, C for warpgroup 1, then O likewise
-  const int loads_per_tile = (P.write_e ? 16 : 8) * NWG;
+  // (C | O) x consumer warpgroup x 4 K blocks x NSTAGE chunks: C for warpgroup 0, C for warpgroup 1, then O likewise
+  const int loads_per_tile = (P.write_e ? 2 : 1) * NWG * 4 * NSTAGE;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < NSTAGE; ++s) {
@@ -335,11 +342,13 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
           const int s = u % NSTAGE;
           mbar_wait(&empty[s], ((u / NSTAGE) & 1) ^ 1, P.error_flag, 1);
           mbar_arrive_expect_tx(&full[s], TC_B_BYTES);
-          // hi, lo of C, then of O; linear mode: hi, lo of block (tile & 3) of U|V|A|B, or of the one embedding
+          // C, then O; linear mode: block (tile & 3) of U|V|A|B, or the one embedding.  Stage s of a K block holds the
+          // hi (s < NSTAGE / 2) or lo rows at K offset (s % (NSTAGE / 2)) * TC_KCH.
           const int row = (lin ? P.lin_w_row + (P.lin_nb == 4 ? (tile & 3) : 0) * W_MAT_ROWS
-                               : P.w_row_base + (i >= 8 * NWG ? w_row_O(0) - w_row_C(0) : 0)) +
-                          (i & 1) * W_LO_ROWS;
-          tma_load_2d(smem_base + Cfg::OFF_B + s * TC_B_BYTES, &wmap, &full[s], ((i >> 1) & 3) * TC_KCH, row);
+                               : P.w_row_base + (i >= 4 * NSTAGE * NWG ? w_row_O(0) - w_row_C(0) : 0)) +
+                          (s >= NSTAGE / 2 ? W_LO_ROWS : 0);
+          const int k = ((i / NSTAGE) & 3) * TC_KBLK + (s % (NSTAGE / 2)) * TC_KCH;
+          tma_load_2d(smem_base + Cfg::OFF_B + s * TC_B_BYTES, &wmap, &full[s], k, row);
         }
       }
     }
@@ -359,18 +368,14 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
   const float** w_tau = s_tau + wg * WG_ROWS;
   auto wg_bar = [&] { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); };
   const int n_rows = lin ? P.lin_rows : P.g.E;
-  // Chunks this warpgroup has read.  With two consumer warpgroups the ring also carries the other warpgroup's 8 chunks
-  // between two GEMMs of this one; 8 chunks fill each stage an even number of times, so the stage and the parity of a
-  // chunk follow from this count alone.
-  uint32_t u = 0;
   float acc[128];
 
   // Turn-taking of the two consumer warpgroups (named barriers 3 and 4, one per warpgroup).  GEMMs run in ring order,
   // warpgroup 0's and warpgroup 1's alternating, so each warpgroup's GEMM is preceded by one of the other's.  A warpgroup
   // enters its GEMM on its own barrier (bar.sync, 256 threads), which the other warpgroup's bar.arrive completes once its
-  // own GEMM has drained.  By then the ring has delivered the two chunks before this GEMM's first two, so each stage is
-  // at most one phase ahead of a parity wait on it.  These waits need no watchdog: the other warpgroup reaches its
-  // bar.arrive through bounded mbarrier waits only.  Warpgroup 1 opens warpgroup 0's first turn; its pass after its last
+  // own GEMM has drained.  By then the ring has delivered the NSTAGE chunks before this GEMM's first NSTAGE, so each
+  // stage is at most one phase ahead of a parity wait on it.  These waits need no watchdog: the other warpgroup reaches
+  // its bar.arrive through bounded mbarrier waits only.  Warpgroup 1 opens warpgroup 0's first turn; its pass after its last
   // GEMM is left unmatched when the CTA exits.  (Taking it after the tile loop made ptxas spill three times as much.)
   auto turn_wait = [&] {
     if constexpr (NWG == 2) asm volatile("bar.sync %0, 256;" ::"r"(3 + wg) : "memory");
@@ -398,7 +403,11 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
     }
   };
 
-  // 8 weight chunks (4 K-chunks x hi, lo) against this warpgroup's A operand (hi, lo at chunk 2 kc, 2 kc + 1).
+  // 4 K blocks x NSTAGE weight chunks against this warpgroup's A operand (hi, lo of K block kc at chunk 2 kc, 2 kc + 1).
+  // Per K block: a_hi * b_hi and a_lo * b_hi for k16 steps 0..3 (the hi chunks), then a_hi * b_lo (the lo chunks).
+  // Chunk s of K block kc sits in stage s, and this warpgroup's GEMMs take 4 NSTAGE ring positions each (so do the
+  // other warpgroup's in between), so its full barrier completes its phase with parity kc & 1.  The stage stays a
+  // compile-time constant: the K-block loop is rolled, the chunks inside it are not.
   // One wgmma group stays in flight across chunk boundaries: chunk i is issued before chunk i - 1's stage is released,
   // so the wait for chunk i + 1's weights overlaps chunk i's tensor work.  The wgmmas still run in issue order on acc.
   // The time spent waiting for the turn is left out of every phase slot.
@@ -408,34 +417,35 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
     if constexpr (TIMED) t_mark = (uint32_t)clock();
     acc_fence(acc);
     wgmma_fence();
-    int s_prev = 0;
+#pragma unroll 1
+    for (int kc = 0; kc < 4; ++kc) {
+      const uint32_t ahi = a_base + kc * 2 * TC_A_CHUNK, alo = ahi + TC_A_CHUNK;
 #pragma unroll
-    for (int i = 0; i < 8; ++i, ++u) {
-      const int s = u % NSTAGE;
-      uint32_t w0 = 0;
-      if constexpr (TIMED) w0 = (uint32_t)clock();
-      mbar_wait(&full[s], (u / NSTAGE) & 1, P.error_flag, 2);
-      if constexpr (TIMED) waited += (uint32_t)clock() - w0;
-      const uint32_t b = smem_base + Cfg::OFF_B + s * TC_B_BYTES;
-      const uint32_t ahi = a_base + (i >> 1) * 2 * TC_A_CHUNK, alo = ahi + TC_A_CHUNK;
+      for (int s = 0; s < NSTAGE; ++s) {
+        uint32_t w0 = 0;
+        if constexpr (TIMED) w0 = (uint32_t)clock();
+        mbar_wait(&full[s], kc & 1, P.error_flag, 2);
+        if constexpr (TIMED) waited += (uint32_t)clock() - w0;
+        const uint32_t b = smem_base + Cfg::OFF_B + s * TC_B_BYTES;
+        const bool b_hi = s < NSTAGE / 2;
 #pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        const uint64_t db = wgmma_desc_sw128(b + ks * 32);
-        wgmma_bf16(acc, wgmma_desc_sw128(ahi + ks * 32), db, (i | ks) ? 1u : 0u);   // hi*hi (B hi) or hi*lo (B lo)
-        if ((i & 1) == 0) wgmma_bf16(acc, wgmma_desc_sw128(alo + ks * 32), db, 1u);   // lo*hi
-      }
-      wgmma_commit();
-      if (i > 0) {
-        wgmma_wait<1>();   // chunk i - 1 has been read
+        for (int k = 0; k < TC_KCH / 16; ++k) {
+          const int ks = (s % (NSTAGE / 2)) * (TC_KCH / 16) + k;   // k16 step inside the K block
+          const uint64_t db = wgmma_desc_sw64(b + k * 32);
+          // hi*hi (B hi) or hi*lo (B lo); only the GEMM's very first wgmma overwrites acc
+          wgmma_bf16(acc, wgmma_desc_sw128(ahi + ks * 32), db, (b_hi && ks == 0) ? (uint32_t)(kc != 0) : 1u);
+          if (b_hi) wgmma_bf16(acc, wgmma_desc_sw128(alo + ks * 32), db, 1u);   // lo*hi
+        }
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous chunk has been read (nothing to wait for at the GEMM's first)
         __syncwarp();
-        if (lane == 0) mbar_arrive(&empty[s_prev]);
+        if (lane == 0 && (s > 0 || kc > 0)) mbar_arrive(&empty[(s + NSTAGE - 1) % NSTAGE]);
       }
-      s_prev = s;
     }
     wgmma_wait<0>();
     acc_fence(acc);
     __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[s_prev]);
+    if (lane == 0) mbar_arrive(&empty[NSTAGE - 1]);
     turn_pass();
     if constexpr (TIMED) {
       const uint32_t now = (uint32_t)clock();
@@ -790,7 +800,7 @@ inline int tc_init(TcState* st, int num_sms) {
 }
 
 // One tensor map over the whole bf16 weight arena at `arena` (w_arena_rows(L) rows of 256 K, layout above).
-// Box = 64 K x 256 rows, 128-byte swizzle.
+// Box = 32 K x 256 rows, 64-byte swizzle: one weight chunk.
 inline int tc_bind_weights(TcState* st, const uint16_t* arena, int L) {
   void* fn = nullptr;
   cudaDriverEntryPointQueryResult qres;
@@ -805,7 +815,7 @@ inline int tc_bind_weights(TcState* st, const uint16_t* arena, int L) {
   cuuint32_t box[2] = {(cuuint32_t)TC_KCH, 256u};
   cuuint32_t estr[2] = {1u, 1u};
   CUresult r = ((PFN_encodeTiled)fn)(&st->wmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)arena, gdim,
-                                     gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                                     gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B,
                                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     st->err = "cuTensorMapEncodeTiled failed with CUresult " + std::to_string((int)r);

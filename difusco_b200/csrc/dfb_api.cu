@@ -57,6 +57,16 @@ struct dfb_ctx {
   // ---- workspace ----
   DevBuf e, h, h0, uvab, uvab0, partials, feat, tvec, gn_part, gn_stats, d_points, d_xt, d_u;
   DevBuf opt_points, opt_tours, opt_pos, opt_dnext, opt_cand, opt_best, opt_table;   // 2-opt (row f3)
+  // ---- host-input staging (pinned) ----
+  // dfb_prepare_graph and dfb_set_points copy host inputs into one of two pinned slots (guarded by an event each, like
+  // the step slots below) and upload from there, so they return without waiting for work already on the stream and the
+  // caller's buffer is free as soon as they return.  A slot grows (cudaFreeHost / cudaHostAlloc) only for a graph
+  // larger than any staged before.
+  static constexpr int UPLOAD_SLOTS = 2;
+  char* h_upload[UPLOAD_SLOTS] = {nullptr, nullptr};
+  size_t h_upload_cap[UPLOAD_SLOTS] = {0, 0};
+  cudaEvent_t upload_ev[UPLOAD_SLOTS] = {nullptr, nullptr};
+  int upload_next = 0;
   // ---- step staging (pinned) + captured loop ----
   // dfb_denoise_step / dfb_denoise never allocate, never synchronise the host with the stream and never touch the
   // heap after the first call of a shape: timesteps and per-step parameters go through two pinned staging slots
@@ -102,6 +112,10 @@ struct dfb_ctx {
     if (loop_stream) cudaStreamDestroy(loop_stream);
     if (loop_in) cudaEventDestroy(loop_in);
     if (loop_out) cudaEventDestroy(loop_out);
+    for (int i = 0; i < UPLOAD_SLOTS; ++i) {
+      if (h_upload[i]) cudaFreeHost(h_upload[i]);
+      if (upload_ev[i]) cudaEventDestroy(upload_ev[i]);
+    }
     for (int i = 0; i < STAGE_SLOTS; ++i) {
       if (h_tvals[i]) cudaFreeHost(h_tvals[i]);
       if (h_steps[i]) cudaFreeHost(h_steps[i]);
@@ -135,9 +149,13 @@ struct dfb_ctx {
       FAIL(ctx, DFB_E_CUDA, "kernel launch failed: %s (%s:%d)", cudaGetErrorString(_e), __FILE__, __LINE__); \
   } while (0)
 
-static int ensure(dfb_ctx* ctx, DevBuf& b, size_t bytes) {
+// Grows b to at least `bytes`.  cudaFree / cudaMalloc synchronise the device, which happens only for a graph (or a
+// 2-opt call) larger than any before.  A captured loop bakes the pointers of the buffers it reads, so growing one of
+// those makes it stale (buf_gen); loop_reads = false is for buffers no loop reads (2-opt, point staging), whose growth
+// must not cost a re-capture.
+static int ensure(dfb_ctx* ctx, DevBuf& b, size_t bytes, bool loop_reads = true) {
   if (bytes <= b.cap) return DFB_OK;
-  ctx->buf_gen++;   // a captured loop that baked the old pointer is stale
+  if (loop_reads) ctx->buf_gen++;   // a captured loop that baked the old pointer is stale
   if (b.p) cudaFree(b.p);
   b.p = nullptr;
   b.cap = 0;
@@ -159,6 +177,60 @@ static int ensure(dfb_ctx* ctx, DevBuf& b, size_t bytes) {
     int _r = ensure(ctx, buf, bytes);            \
     if (_r) return _r;                           \
   } while (0)
+#define ENS_NOLOOP(ctx, buf, bytes)              \
+  do {                                           \
+    int _r = ensure(ctx, buf, bytes, false);     \
+    if (_r) return _r;                           \
+  } while (0)
+
+// One host-to-device copy of a host-input upload, into a context buffer (resolved when the copy is enqueued, so the
+// buffer may grow between upload_reserve and upload_send).
+struct Upload {
+  DevBuf* dst;
+  const void* src;
+  size_t bytes;
+};
+
+static size_t upload_padded(size_t b) { return (b + 15) & ~(size_t)15; }
+
+// Takes the next pinned upload slot and makes room for `ups` in it.  Waits (host side) only for the uploads of the call
+// that used the slot two calls ago.  Called before the call grows or changes any device state, so that a failed
+// cudaHostAlloc leaves the context as it was.  -> *slot
+static int upload_reserve(dfb_ctx* ctx, const std::vector<Upload>& ups, int* slot) {
+  size_t total = 0;
+  for (const Upload& u : ups) total += upload_padded(u.bytes);
+  const int sl = ctx->upload_next;
+  CK(ctx, cudaEventSynchronize(ctx->upload_ev[sl]));
+  if (total > ctx->h_upload_cap[sl]) {
+    if (ctx->h_upload[sl]) cudaFreeHost(ctx->h_upload[sl]);
+    ctx->h_upload[sl] = nullptr;
+    ctx->h_upload_cap[sl] = 0;
+    const size_t want = total + (total >> 3);
+    cudaError_t e = cudaHostAlloc((void**)&ctx->h_upload[sl], want, cudaHostAllocDefault);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      ctx->h_upload[sl] = nullptr;
+      FAIL(ctx, DFB_E_NOMEM, "cudaHostAlloc(%zu bytes) for host-input staging failed: %s", want, cudaGetErrorString(e));
+    }
+    ctx->h_upload_cap[sl] = want;
+  }
+  ctx->upload_next = (sl + 1) % dfb_ctx::UPLOAD_SLOTS;
+  *slot = sl;
+  return DFB_OK;
+}
+
+// Copies every ups[i].src into the reserved slot and enqueues its upload to ups[i].dst on st; the caller's buffers are
+// consumed when it returns.
+static int upload_send(dfb_ctx* ctx, int slot, const std::vector<Upload>& ups, cudaStream_t st) {
+  char* p = ctx->h_upload[slot];
+  for (const Upload& u : ups) {
+    memcpy(p, u.src, u.bytes);
+    CK(ctx, cudaMemcpyAsync(u.dst->p, p, u.bytes, cudaMemcpyHostToDevice, st));
+    p += upload_padded(u.bytes);
+  }
+  CK(ctx, cudaEventRecord(ctx->upload_ev[slot], st));
+  return DFB_OK;
+}
 
 static bool is_device_ptr(const void* p) {
   cudaPointerAttributes a;
@@ -223,6 +295,13 @@ extern "C" int dfb_create(dfb_ctx** out, int device) {
         (e = cudaHostAlloc((void**)&ctx->h_steps[i], dfb_ctx::MAX_STEPS * sizeof(StepParams), cudaHostAllocDefault)) != cudaSuccess ||
         (e = cudaEventCreateWithFlags(&ctx->stage_ev[i], cudaEventDisableTiming)) != cudaSuccess) {
       g_create_error = std::string("pinned staging: ") + cudaGetErrorString(e);
+      delete ctx;
+      return DFB_E_CUDA;
+    }
+  }
+  for (int i = 0; i < dfb_ctx::UPLOAD_SLOTS; ++i) {
+    if ((e = cudaEventCreateWithFlags(&ctx->upload_ev[i], cudaEventDisableTiming)) != cudaSuccess) {
+      g_create_error = std::string("host-input staging: ") + cudaGetErrorString(e);
       delete ctx;
       return DFB_E_CUDA;
     }
@@ -470,7 +549,7 @@ extern "C" int dfb_set_aggregation(dfb_ctx* ctx, int mode) {
 // ================================================================================================
 // dfb_prepare_graph (node_ptr null: gn_segments equal row blocks) and dfb_prepare_graph_instances (node_ptr[n_inst + 1]:
 // one segment per instance).  Every argument is checked before any context state changes, so a rejected call leaves
-// the previously prepared graph in use.
+// the previously prepared graph in use.  A call that fails for want of memory after that leaves no graph prepared.
 static int prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_t V64, int64_t E64, int gn_segments,
                          int n_inst, const int64_t* node_ptr, cudaStream_t st) {
   if (!ctx) return DFB_E_INVALID;
@@ -575,31 +654,27 @@ static int prepare_graph(dfb_ctx* ctx, const int64_t* edge_index, int64_t V64, i
   }
   gpair[nG] = np;
 
-  ENS(ctx, ctx->d_row, (size_t)E * 4);
-  ENS(ctx, ctx->d_col, (size_t)E * 4);
-  ENS(ctx, ctx->d_rowptr, ((size_t)V + 1) * 4);
-  ENS(ctx, ctx->d_grp_first, (size_t)nG * 4);
-  ENS(ctx, ctx->d_grp_pair, ((size_t)nG + 1) * 4);
-  CK(ctx, cudaMemcpyAsync(ctx->d_row.p, row.data(), (size_t)E * 4, cudaMemcpyHostToDevice, st));
-  CK(ctx, cudaMemcpyAsync(ctx->d_col.p, col.data(), (size_t)E * 4, cudaMemcpyHostToDevice, st));
-  CK(ctx, cudaMemcpyAsync(ctx->d_rowptr.p, rowptr.data(), ((size_t)V + 1) * 4, cudaMemcpyHostToDevice, st));
-  CK(ctx, cudaMemcpyAsync(ctx->d_grp_first.p, gfirst.data(), (size_t)nG * 4, cudaMemcpyHostToDevice, st));
-  CK(ctx, cudaMemcpyAsync(ctx->d_grp_pair.p, gpair.data(), ((size_t)nG + 1) * 4, cudaMemcpyHostToDevice, st));
-  if (!sorted) {
-    ENS(ctx, ctx->d_perm, (size_t)E * 4);
-    CK(ctx, cudaMemcpyAsync(ctx->d_perm.p, perm.data(), (size_t)E * 4, cudaMemcpyHostToDevice, st));
-  }
-  ENS(ctx, ctx->d_seg_start, ((size_t)S + 1) * 4);
-  ENS(ctx, ctx->d_seg_blk_first, ((size_t)S + 1) * 4);
-  ENS(ctx, ctx->d_gn_blk, (size_t)nb * sizeof(int2));
-  CK(ctx, cudaMemcpyAsync(ctx->d_seg_start.p, seg_start.data(), ((size_t)S + 1) * 4, cudaMemcpyHostToDevice, st));
-  CK(ctx, cudaMemcpyAsync(ctx->d_seg_blk_first.p, blk_first.data(), ((size_t)S + 1) * 4, cudaMemcpyHostToDevice, st));
-  CK(ctx, cudaMemcpyAsync(ctx->d_gn_blk.p, gn_blk.data(), (size_t)nb * sizeof(int2), cudaMemcpyHostToDevice, st));
-  if (!local.empty()) {
-    ENS(ctx, ctx->d_local, (size_t)E * 4);
-    CK(ctx, cudaMemcpyAsync(ctx->d_local.p, local.data(), (size_t)E * 4, cudaMemcpyHostToDevice, st));
-  }
-  CK(ctx, cudaStreamSynchronize(st));   // host vectors go out of scope
+  // stream-ordered through pinned staging: a loop already enqueued on the previous graph still reads its tables, and
+  // the host vectors may go out of scope without waiting for the stream
+  std::vector<Upload> ups = {
+      {&ctx->d_row, row.data(), (size_t)E * 4},
+      {&ctx->d_col, col.data(), (size_t)E * 4},
+      {&ctx->d_rowptr, rowptr.data(), ((size_t)V + 1) * 4},
+      {&ctx->d_grp_first, gfirst.data(), (size_t)nG * 4},
+      {&ctx->d_grp_pair, gpair.data(), ((size_t)nG + 1) * 4},
+      {&ctx->d_seg_start, seg_start.data(), ((size_t)S + 1) * 4},
+      {&ctx->d_seg_blk_first, blk_first.data(), ((size_t)S + 1) * 4},
+      {&ctx->d_gn_blk, gn_blk.data(), (size_t)nb * sizeof(int2)}};
+  if (!sorted) ups.push_back({&ctx->d_perm, perm.data(), (size_t)E * 4});
+  if (!local.empty()) ups.push_back({&ctx->d_local, local.data(), (size_t)E * 4});
+  int slot;
+  int r = upload_reserve(ctx, ups, &slot);
+  if (r) return r;
+  // From here on a failure (device memory exhausted) leaves no graph prepared rather than tables in freed buffers.
+  ctx->graph_ready = ctx->points_ready = false;
+  for (const Upload& u : ups) ENS(ctx, *u.dst, u.bytes);
+  r = upload_send(ctx, slot, ups, st);
+  if (r) return r;
   GraphDev& g = ctx->g;
   g.V = V; g.E = E;
   g.row = (const int*)ctx->d_row.p; g.col = (const int*)ctx->d_col.p;
@@ -688,8 +763,14 @@ extern "C" int dfb_set_points(dfb_ctx* ctx, const float* points, void* stream_) 
   const int V = ctx->g.V;
   const float* dp = points;
   if (!is_device_ptr(points)) {
-    ENS(ctx, ctx->d_points, (size_t)V * 2 * sizeof(float));
-    CK(ctx, cudaMemcpyAsync(ctx->d_points.p, points, (size_t)V * 2 * sizeof(float), cudaMemcpyHostToDevice, st));
+    const std::vector<Upload> ups = {{&ctx->d_points, points, (size_t)V * 2 * sizeof(float)}};
+    int slot;
+    int r = upload_reserve(ctx, ups, &slot);
+    if (r) return r;
+    ctx->points_ready = false;   // a failure below leaves no points rather than the previous ones
+    ENS_NOLOOP(ctx, ctx->d_points, ups[0].bytes);
+    r = upload_send(ctx, slot, ups, st);
+    if (r) return r;
     dp = (const float*)ctx->d_points.p;
   }
   const int CH = 65536;
@@ -1346,7 +1427,7 @@ extern "C" int dfb_knn_graph(dfb_ctx* ctx, const double* points, int64_t num_nod
     // KDTree rejects NaN and inf; device-resident points are the caller's to check (knn_edge_index_gpu does)
     for (int64_t i = 0; i < 2 * num_nodes; ++i)
       if (!std::isfinite(points[i])) FAIL(ctx, DFB_E_INVALID, "kNN graph: non-finite coordinate of node %lld", (long long)(i / 2));
-    ENS(ctx, ctx->d_points, (size_t)num_nodes * 2 * sizeof(double));
+    ENS_NOLOOP(ctx, ctx->d_points, (size_t)num_nodes * 2 * sizeof(double));
     CK(ctx, cudaMemcpyAsync(ctx->d_points.p, points, (size_t)num_nodes * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
     dp = (const double*)ctx->d_points.p;
   }
@@ -1411,13 +1492,13 @@ static int two_opt_run(dfb_ctx* ctx, const double* points, const int64_t* node_p
   std::vector<char> table(inst_bytes + sizeof(int));
   memcpy(table.data(), insts.data(), inst_bytes);
   memcpy(table.data() + inst_bytes, &running, sizeof(int));
-  ENS(ctx, ctx->opt_points, (size_t)V * 2 * sizeof(double));
-  ENS(ctx, ctx->opt_tours, (size_t)entries * sizeof(long long));
-  ENS(ctx, ctx->opt_pos, (size_t)entries * 2 * sizeof(double));
-  ENS(ctx, ctx->opt_dnext, (size_t)(entries - n_tours) * sizeof(double));
-  ENS(ctx, ctx->opt_cand, (size_t)items * sizeof(TwoOptCand));
-  ENS(ctx, ctx->opt_best, (size_t)n_tours * sizeof(TwoOptCand));
-  ENS(ctx, ctx->opt_table, table.size());
+  ENS_NOLOOP(ctx, ctx->opt_points, (size_t)V * 2 * sizeof(double));
+  ENS_NOLOOP(ctx, ctx->opt_tours, (size_t)entries * sizeof(long long));
+  ENS_NOLOOP(ctx, ctx->opt_pos, (size_t)entries * 2 * sizeof(double));
+  ENS_NOLOOP(ctx, ctx->opt_dnext, (size_t)(entries - n_tours) * sizeof(double));
+  ENS_NOLOOP(ctx, ctx->opt_cand, (size_t)items * sizeof(TwoOptCand));
+  ENS_NOLOOP(ctx, ctx->opt_best, (size_t)n_tours * sizeof(TwoOptCand));
+  ENS_NOLOOP(ctx, ctx->opt_table, table.size());
   double* d_points = (double*)ctx->opt_points.p;
   long long* d_tours = (long long*)ctx->opt_tours.p;
   double* d_pos = (double*)ctx->opt_pos.p;

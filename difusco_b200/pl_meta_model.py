@@ -231,7 +231,9 @@ class COMetaModel(_Base):
           [int(s) for s in record_steps]
       if any(s < 0 or s >= steps for s in rec) or any(b <= a for a, b in zip(rec, rec[1:])):
         raise ValueError(f"record_steps must be strictly increasing and inside [0, {steps}): {rec}")
-    d_seeds = None if seeds is None else torch.from_numpy(seeds.view(np.int64)).to(xt.device)
+    # pinned and non-blocking: enqueuing a loop never waits for the loops already on the stream
+    d_seeds = None if seeds is None else \
+        torch.from_numpy(seeds.view(np.int64)).pin_memory().to(xt.device, non_blocking=True)
     if record_steps is None:
       if d_seeds is None:
         ctx.denoise(mode, xt.data_ptr(), t1s, consts, lasts, None, seed, stream)
@@ -254,6 +256,79 @@ class COMetaModel(_Base):
       ctx.denoise_instances(mode, xt.data_ptr(), t1s, consts, lasts, d_seeds.data_ptr(), seeds.size, rec, *ptrs,
                             stream)
     return xt, trace
+
+  # ---------------------------------------------------------------------------------------
+  # solving a stream of batches: solve_batch is the one-batch case of solve_batches
+  # ---------------------------------------------------------------------------------------
+  # Where a batch's 2-opt runs: on a second, higher-priority stream beside the next batch's loops (True), or on the
+  # loops' stream, where it follows the next batch's loops already enqueued there (False).  Chosen by measurement
+  # (DESIGN §4.2, "Solving a batch"); not an option.
+  _two_opt_beside_loop = True
+
+  def solve_batch(self, batch, seeds, split="test"):
+    """test_step for every instance of a collated batch at once (see _solve_enqueue of the task model).  seeds: one int
+    per instance; instance i's round seeds and initial noise come from a torch.Generator seeded with seeds[i] alone and
+    the sampling is keyed per instance, so its result does not depend on the other instances of the batch.  Returns one
+    metrics dict per instance with test_step's keys, and logs them as n test_step calls would."""
+    return next(self.solve_batches([batch], [seeds], split))
+
+  def solve_batches(self, batches, seeds, split="test"):
+    """Generator: for each batch of `batches` (any iterable of collated batches, e.g. a DataLoader), in order, yields
+    exactly what solve_batch(batch, seeds[k], split) returns, logs what it logs and sets its last_* artefacts when it
+    yields.  seeds: one seed list per batch.
+
+    The host work of one batch is hidden behind the next batch's loops: batch k + 1's inputs are prepared and its
+    denoise loops enqueued before batch k is decoded, heat maps reach the host through pinned buffers and events, and
+    batch k's 2-opt runs beside batch k + 1's loops.  An exception of batch k (a malformed batch, bad seeds, fewer or
+    more seed lists than batches) is raised when batch k is reached, after batches < k were yielded; the model stays
+    usable."""
+    batches, seed_lists = iter(batches), iter(seeds)
+    job = self._next_solve_job(batches, seed_lists)
+    while job is not None:
+      if isinstance(job, Exception):
+        raise job
+      following = self._next_solve_job(batches, seed_lists)
+      yield self._solve_finish(job, split)
+      job = following
+
+  def _next_solve_job(self, batches, seed_lists):
+    """_solve_enqueue of the next batch -> its job, None after the last batch, or the exception it raised."""
+    end = object()
+    try:
+      batch, seeds = next(batches, end), next(seed_lists, end)
+      if batch is end:
+        if seeds is not end:
+          raise ValueError("solve_batches: more seed lists than batches")
+        return None
+      if seeds is end:
+        raise ValueError("solve_batches: fewer seed lists than batches")
+      return self._solve_enqueue(batch, seeds)
+    except Exception as e:   # raised when this batch is reached, after the earlier ones were yielded
+      return e
+
+  @staticmethod
+  def _pinned_to_device(x, dev):
+    """Host tensor -> device copy that does not wait for the work already on the stream."""
+    return x.pin_memory().to(dev, non_blocking=True)
+
+  @staticmethod
+  def _to_host_async(x):
+    """Device tensor -> (pinned host copy, event recorded after the copy); wait on the event before reading it."""
+    host = torch.empty(x.shape, dtype=x.dtype, pin_memory=True)
+    host.copy_(x, non_blocking=True)
+    ev = torch.cuda.Event()
+    ev.record()
+    return host, ev
+
+  def _two_opt_stream(self, dev):
+    """The stream a batch's 2-opt runs on (see _two_opt_beside_loop)."""
+    if not self._two_opt_beside_loop:
+      return torch.cuda.current_stream(dev)
+    s = self.__dict__.get("_dfb_two_opt_stream")
+    if s is None or s.device != dev:
+      s = torch.cuda.Stream(dev, priority=-1)   # higher priority: its short launches go first at launch boundaries
+      self.__dict__["_dfb_two_opt_stream"] = s
+    return s
 
   @staticmethod
   def _solve_seeds(seeds, n):

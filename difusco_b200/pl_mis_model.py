@@ -7,7 +7,8 @@
 Greedy MIS decoding (mis_decode_np, :194-196; SURVEY 8f row f4) is `difusco_b200.utils.mis_utils.mis_decode_np`,
 applied by test_step exactly as the reference does (best of all samples -> `{split}/solved_cost`).
 solve_batch(batch, seeds, split='test') runs test_step for every graph of a collated batch at once, each graph's result
-independent of the rest of the batch.
+independent of the rest of the batch; solve_batches(batches, seeds, split='test') runs it over a stream of batches with
+each batch's decode hidden behind the next batch's loops (COMetaModel.solve_batches).
 """
 import numpy as np
 import torch
@@ -44,7 +45,7 @@ class MISModel(COMetaModel):
     steps = steps or self.args.inference_diffusion_steps
     with torch.no_grad():
       dev = self.model._device()
-      self.model.set_graph(edge_index.long().to(dev), xt.shape[0], 1, node_ptr)
+      self.model.set_graph(edge_index.long(), xt.shape[0], 1, node_ptr)   # host edges: staged without a wait
       x = xt.reshape(-1).float().contiguous().to(dev).clone()
       return self._fused_loop(x, steps, seed, record_steps, instance_seeds)
 
@@ -87,14 +88,12 @@ class MISModel(COMetaModel):
     self.last_solved_cost = best_solved_cost
     return metrics
 
-  def solve_batch(self, batch, seeds, split="test"):
-    """test_step for every graph of a collated batch (index, graph, point_indicator): graph.x / graph.edge_index
+  def _solve_enqueue(self, batch, seeds):
+    """solve_batch's device half for a collated batch (index, graph, point_indicator): graph.x / graph.edge_index
     concatenated in graph order with node offsets, point_indicator the node counts.  Each graph's parallel_sampling
-    replicas share one GroupNorm as in test_step; all graphs run in one fused loop per sequential round, then
-    mis_decode_np per graph.  seeds: one int per graph; its round seeds and initial noise come from a torch.Generator
-    seeded with seeds[i] alone and the sampling is keyed per graph, so its result does not depend on the other graphs.
-    Returns one metrics dict per graph with test_step's keys, and logs them as n test_step calls would."""
-    import scipy.sparse
+    replicas share one GroupNorm as in test_step; all graphs run in one fused loop per sequential round, enqueued with
+    its labels copied to pinned host memory.  Checks the batch and the seeds before any device work, and waits for no
+    earlier loop.  -> the job _solve_finish decodes."""
     _, graph_data, point_indicator = batch
     labels = graph_data.x.reshape(-1)
     edge_index = graph_data.edge_index.reshape(2, -1)
@@ -111,19 +110,31 @@ class MISModel(COMetaModel):
     dev = self.model._device()
     local = [np.ascontiguousarray(ei[:, owner == i] - node0[i]) for i in range(len(sizes))]
     ptr = np.concatenate([[0], np.cumsum([P * n for n in sizes])]).astype(np.int64)
-    edges = torch.cat([self.duplicate_edge_index(torch.from_numpy(e).to(dev), n, dev) + int(ptr[i])
+    edges = torch.cat([self.duplicate_edge_index(torch.from_numpy(e), n, "cpu") + int(ptr[i])
                        for i, (e, n) in enumerate(zip(local, sizes))], 1)
-    samples = [[] for _ in sizes]
+    outs = []
     for _ in range(rounds):
       round_seeds, noise = [], []
       for g, n in zip(gens, sizes):
         round_seeds.append(self._round_seed(g))
         z = torch.randn(P * n, generator=g)
         noise.append((z > 0).float() if self.diffusion_type != "gaussian" else z)
-      xt = self.denoise_labels(edges, torch.cat(noise), node_ptr=ptr, instance_seeds=round_seeds)
-      xt = xt.float().cpu().detach().numpy()
+      xt = self._pinned_to_device(torch.cat(noise), dev)
+      outs.append(self._to_host_async(self.denoise_labels(edges, xt, node_ptr=ptr, instance_seeds=round_seeds)))
+    return dict(sizes=sizes, local=local, ptr=ptr, outs=outs,
+                gt=[labels[node0[i]:node0[i + 1]].cpu().numpy().sum() for i in range(len(sizes))])
+
+  def _solve_finish(self, job, split):
+    """solve_batch's host half: mis_decode_np per graph and sample, the metrics and the logs."""
+    import scipy.sparse
+    P, rounds = self.args.parallel_sampling, self.args.sequential_sampling
+    sizes, local = job["sizes"], job["local"]
+    samples = [[] for _ in sizes]
+    for host, ev in job["outs"]:
+      ev.synchronize()
+      xt = host.float().numpy()
       xt = xt * 0.5 + 0.5 if self.diffusion_type == "gaussian" else xt + 1e-6
-      for i, part in enumerate(np.split(xt, ptr[1:-1])):
+      for i, part in enumerate(np.split(xt, job["ptr"][1:-1])):
         samples[i].append(part)
     out, costs = [], []
     for i, n in enumerate(sizes):
@@ -131,7 +142,7 @@ class MISModel(COMetaModel):
       predict_labels = np.concatenate(samples[i], axis=0)
       solved = [mis_decode_np(pl, adj_mat) for pl in np.split(predict_labels, rounds * P)]
       best = np.max([sol.sum() for sol in solved])
-      metrics = {f"{split}/gt_cost": labels[node0[i]:node0[i + 1]].cpu().numpy().sum()}
+      metrics = {f"{split}/gt_cost": job["gt"][i]}
       # batch_size=1: each value is one graph's, as test_step logs it; Lightning would otherwise weight it by the size
       # it infers from the collated batch
       for k, v in metrics.items():

@@ -6,7 +6,9 @@ Same method names and signatures on the denoise path:
   gaussian_denoise_step(points, xt, t, device, edge_index=None, target_t=None)      :140-151
   test_step(batch, batch_idx, split='test')                                   :153-256
 plus solve_batch(batch, seeds, split='test'): test_step for the n instances of a collated batch in one fused loop per
-sequential round and one multi-instance 2-opt, each instance's result independent of the rest of the batch.
+sequential round and one multi-instance 2-opt, each instance's result independent of the rest of the batch, and
+solve_batches(batches, seeds, split='test'): solve_batch over a stream of batches, with each batch's decode hidden behind
+the next batch's loops (COMetaModel.solve_batches).
 test_step runs the reference's loop (:185-222) as ONE fused device loop, then the reference's decode
 (:227-256; SURVEY 8f rows f2/f3): merge_tours (host C++), batched 2-opt (CUDA), TSPEvaluator - and returns the
 reference's metrics dict.  `--save_numpy_heatmap` (:224-225, :258-267) is honoured.
@@ -39,17 +41,18 @@ class TSPModel(COMetaModel):
 
   # ------------------------------------------------------------------------------------
   def _prepare(self, points, edge_index, device, node_ptr=None):
-    """Make self.model's engine hold this call's graph + coordinates; returns dense batch B or 0."""
+    """Make self.model's engine hold this call's graph + coordinates; returns dense batch B or 0.  Host tensors go to
+    the engine as they are: it stages them through pinned memory without waiting for the loops already enqueued."""
     if self.sparse:
       V = points.shape[0]
-      self.model.set_graph(edge_index.long().to(device), V, 1, node_ptr)
-      self.model.set_points(points.float().to(device))
+      self.model.set_graph(edge_index.long(), V, 1, node_ptr)
+      self.model.set_points(points.float())
       return 0
     if node_ptr is not None:
       raise ValueError("node_ptr is for sparse graphs: the dense path already normalises each sample on its own")
     B, V, _ = points.shape
-    self.model.set_graph(self.model._complete_graph(B, V, device), B * V, B)
-    self.model.set_points(points.reshape(B * V, 2).float().to(device))
+    self.model.set_graph(self.model._complete_graph(B, V, torch.device("cpu")), B * V, B)
+    self.model.set_points(points.reshape(B * V, 2).float())
     return B
 
   def _denoise_step(self, points, xt, t, device, edge_index, target_t):
@@ -83,7 +86,7 @@ class TSPModel(COMetaModel):
     steps = steps or self.args.inference_diffusion_steps
     with torch.no_grad():
       dev = self.model._device()
-      self._prepare(points.to(dev), edge_index.to(dev) if edge_index is not None else None, dev, node_ptr)
+      self._prepare(points, edge_index, dev, node_ptr)
       x = xt.reshape(-1).float().contiguous().to(dev).clone()
       if record_steps is None:
         self._fused_loop(x, steps, seed, instance_seeds=instance_seeds)
@@ -190,32 +193,30 @@ class TSPModel(COMetaModel):
       v0, e0 = v0 + n, e0 + e
     return out
 
-  def solve_batch(self, batch, seeds, split="test"):
-    """test_step for every instance of a collated batch: each instance's parallel_sampling replicas in one fused
-    denoise loop per sequential round (the replicas of a sparse instance share one GroupNorm, as in test_step; a dense
-    replica is a sample of its own), then merge_tours per instance and round and one batched_two_opt_instances.
-
-    seeds: one int per instance.  Instance i's round seeds and initial noise come from a torch.Generator seeded with
-    seeds[i] alone and the sampling is keyed per instance, so its tours and metrics do not depend on the other
-    instances of the batch.  Returns one metrics dict per instance with test_step's keys, and logs them as n
-    test_step calls would."""
+  def _solve_enqueue(self, batch, seeds):
+    """solve_batch's device half: each instance's parallel_sampling replicas in one fused denoise loop per sequential
+    round (the replicas of a sparse instance share one GroupNorm, as in test_step; a dense replica is a sample of its
+    own), every round enqueued with its heat map copied to pinned host memory.  Checks the batch and the seeds before
+    any device work, and waits for no earlier loop.  -> the job _solve_finish decodes."""
     if getattr(self.args, "save_numpy_heatmap", False):
       raise NotImplementedError("solve_batch does not save heat maps: use test_step for --save_numpy_heatmap")
     inst = self._instances(batch)
     gens = self._solve_seeds(seeds, len(inst))
     copies, rounds = self.args.parallel_sampling, self.args.sequential_sampling
     dev = self.model._device()
-    np_points = [p.cpu().numpy() for p, _, _ in inst]
+    # copies: _solve_finish runs after the next batch was drawn, and a loader may refill its tensors in place
+    np_points = [p.cpu().numpy().copy() for p, _, _ in inst]
+    np_edges = [None if e is None else e.cpu().numpy().copy() for _, e, _ in inst]
     if self.sparse:
       sizes = [p.shape[0] for p in np_points]
       ptr = np.concatenate([[0], np.cumsum([copies * n for n in sizes])]).astype(np.int64)
-      coords = torch.cat([p.repeat(copies, 1) for p, _, _ in inst])
-      edges = torch.cat([self.duplicate_edge_index(e.to(dev), n, dev) + int(ptr[i])
-                         for i, ((_, e, _), n) in enumerate(zip(inst, sizes))], 1)
-      lens = [copies * e.shape[1] for _, e, _ in inst]
+      coords = torch.cat([p.cpu().repeat(copies, 1) for p, _, _ in inst])
+      edges = torch.cat([self.duplicate_edge_index(torch.from_numpy(e), n, "cpu") + int(ptr[i])
+                         for i, (e, n) in enumerate(zip(np_edges, sizes))], 1)
+      lens = [copies * e.shape[1] for e in np_edges]
     else:
       ptr = None
-      coords = torch.stack([p for p, _, _ in inst]).repeat_interleave(copies, 0)
+      coords = torch.stack([p.cpu() for p, _, _ in inst]).repeat_interleave(copies, 0)
       edges = None
       lens = [copies] * len(inst)
     heats = []
@@ -226,31 +227,43 @@ class TSPModel(COMetaModel):
         shape = (n_el,) if self.sparse else (copies,) + tuple(inst[0][0].shape[:1]) * 2
         z = torch.randn(shape, generator=g)
         noise.append((z > 0).float() if self.diffusion_type != "gaussian" else z)
-      xt = torch.cat(noise)
-      heat = self._heatmap_to_numpy(self.denoise_heatmap(coords, edges, xt, node_ptr=ptr, instance_seeds=round_seeds))
-      heats.append(np.split(heat, np.cumsum(lens)[:-1]))
+      xt = self._pinned_to_device(torch.cat(noise), dev)
+      heats.append(self._to_host_async(self.denoise_heatmap(coords, edges, xt, node_ptr=ptr,
+                                                            instance_seeds=round_seeds)))
+    return dict(dev=dev, gt=[t.copy() for _, _, t in inst], np_points=np_points, np_edges=np_edges, lens=lens, heats=heats)
+
+  def _solve_finish(self, job, split):
+    """solve_batch's host half: merge_tours per instance and round on a thread pool, one batched_two_opt_instances,
+    the metrics and the logs."""
+    copies, rounds = self.args.parallel_sampling, self.args.sequential_sampling
+    np_points, np_edges = job["np_points"], job["np_edges"]
+    heats = []
+    for host, ev in job["heats"]:
+      ev.synchronize()
+      heats.append(np.split(self._heatmap_to_numpy(host), np.cumsum(job["lens"])[:-1]))
     exact = getattr(self.args, "exact_merge", True)
-    jobs = [(i, r) for i in range(len(inst)) for r in range(rounds)]
+    jobs = [(i, r) for i in range(len(np_points)) for r in range(rounds)]
 
     def merge(job):
       i, r = job
-      e = inst[i][1]
-      return merge_tours(heats[r][i], np_points[i], None if e is None else e.cpu().numpy(), sparse_graph=self.sparse,
-                         parallel_sampling=copies, exact=exact)
+      return merge_tours(heats[r][i], np_points[i], np_edges[i], sparse_graph=self.sparse, parallel_sampling=copies,
+                         exact=exact)
 
     from concurrent.futures import ThreadPoolExecutor
     with ThreadPoolExecutor(max_workers=min(len(jobs), os.cpu_count() or 1)) as pool:
       merged = list(pool.map(merge, jobs))
-    refined, iterations = batched_two_opt_instances(
-        [np_points[i].astype("float64") for i, _ in jobs], [np.array(t).astype("int64") for t, _ in merged],
-        max_iterations=getattr(self.args, "two_opt_iterations", 1000), device=dev)
+    dev = job["dev"]
+    with torch.cuda.stream(self._two_opt_stream(dev)):
+      refined, iterations = batched_two_opt_instances(
+          [np_points[i].astype("float64") for i, _ in jobs], [np.array(t).astype("int64") for t, _ in merged],
+          max_iterations=getattr(self.args, "two_opt_iterations", 1000), device=dev)
     out, tours_out, costs = [], [], []
-    for i in range(len(inst)):
+    for i in range(len(np_points)):
       k = [jobs.index((i, r)) for r in range(rounds)]
       solved = np.concatenate([refined[j] for j in k], axis=0)
       scorer = TSPEvaluator(np_points[i])
       best = np.min([scorer.evaluate(solved[s]) for s in range(copies * rounds)])
-      metrics = {f"{split}/gt_cost": scorer.evaluate(inst[i][2]),
+      metrics = {f"{split}/gt_cost": scorer.evaluate(job["gt"][i]),
                  f"{split}/2opt_iterations": iterations[k[-1]], f"{split}/merge_iterations": merged[k[-1]][1]}
       # batch_size=1: each value is one instance's, as test_step logs it; Lightning would otherwise weight it by the
       # size it infers from the collated batch

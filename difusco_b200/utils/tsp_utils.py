@@ -40,9 +40,13 @@ def batched_two_opt_torch(points, tour, max_iterations=1000, device="cuda"):
 def batched_two_opt_instances(points_list, tours_list, max_iterations=1000, device="cuda"):
   """batched_two_opt_torch on many instances in one call: points_list[i] (n_i, 2), tours_list[i] (B_i, n_i + 1) of
   local node ids -> (tours_list, iterations_list), each instance exactly as batched_two_opt_torch on it alone (its own
-  stopping rule and iteration cap)."""
+  stopping rule and iteration cap).  Runs on torch's current stream of the device, so that under
+  `torch.cuda.stream(s)` it runs beside the work of other streams."""
+  import torch
   _cabi.two_opt_instances_arrays(points_list, tours_list)   # argument checks before any device work
-  return _engine(device).two_opt_instances(points_list, tours_list, max_iterations)
+  ctx = _engine(device)
+  return ctx.two_opt_instances(points_list, tours_list, max_iterations,
+                               torch.cuda.current_stream(ctx.device).cuda_stream)
 
 
 def _dense_order(points, heat, edge_index):

@@ -15,6 +15,20 @@
  * dfb_denoise never allocate device or host memory, never synchronise the host with the stream and never read the
  * environment: per-call scalars travel through two pinned staging slots, per-step tables live in device memory, so
  * the step path is CUDA-graph capturable - and dfb_denoise itself replays a captured graph.
+ *
+ * Host inputs do not block: dfb_prepare_graph / dfb_prepare_graph_instances with a HOST edge_index and dfb_set_points
+ * with HOST points copy their inputs (or the tables built from them) into one of two context-owned pinned staging slots
+ * and upload them stream-ordered, so they return without waiting for work already on `stream` (a loop enqueued on the
+ * previous graph still reads the previous tables), and the caller's buffer, pageable or pinned, may be overwritten as
+ * soon as they return.  They wait only when the slot's uploads from two such calls ago have not run yet, and they
+ * synchronise the device when the arena or a staging slot grows (cudaFree / cudaFreeHost), i.e. for a graph larger than
+ * any prepared before (the pinned slot is reserved first: if pinned memory cannot be had the previous graph stays in
+ * use; if device memory cannot, no graph is left prepared).  A DEVICE edge_index is read back to the host to be
+ * validated, which waits for the stream.  The loop calls keep their own rule: their two step-staging slots make each
+ * one wait until the loop three calls before it has finished.
+ * dfb_two_opt / dfb_two_opt_instances share no scratch with the denoise loop: they may run on a stream of their own
+ * beside a loop of the same context (calls still come from one thread), and growing their buffers never makes the
+ * captured loop re-capture.
  */
 #ifndef DIFUSCO_B200_H_
 #define DIFUSCO_B200_H_

@@ -10,7 +10,7 @@ LIB_PATH = os.path.join(HERE, "libdifusco_b200.so")
 
 DFB_OK, DFB_E_INVALID, DFB_E_CUDA, DFB_E_UNSUPPORTED, DFB_E_NOMEM = 0, -1, -2, -3, -4
 CATEGORICAL, GAUSSIAN = 0, 1
-EDGE_IMPL_TC, EDGE_IMPL_FP32, EDGE_IMPL_TC1 = 0, 1, 2
+EDGE_IMPL_TC, EDGE_IMPL_FP32, EDGE_IMPL_TC1, EDGE_IMPL_TC6 = 0, 1, 2, 3
 AGGREGATION = {"sum": 0, "mean": 1, "max": 2}
 HEAD_FORWARD, HEAD_CATEGORICAL, HEAD_GAUSSIAN = 0, 1, 2
 

@@ -41,7 +41,7 @@ struct dfb_ctx {
   int agg_mode = AGG_SUM;
   int edge_impl = DFB_EDGE_IMPL_TC;
   bool phase_timing = false;   // edge layers of the product kernel run through its timed copy (dfb_set_phase_timing)
-  DevBuf wbuf, wbuf16, layers_dev;
+  DevBuf wbuf, wbuf16, wbuf16_3, layers_dev;   // fp32 arena, bf16 hi / lo arena, bf16 third-part arena (TC6)
   std::vector<LayerParams> layers;
   TimeParams tp{};
   HeadParams hp{};
@@ -336,7 +336,8 @@ extern "C" int dfb_destroy(dfb_ctx* ctx) {
 
 extern "C" int dfb_set_edge_impl(dfb_ctx* ctx, int impl) {
   if (!ctx) return DFB_E_INVALID;
-  if (impl != DFB_EDGE_IMPL_TC && impl != DFB_EDGE_IMPL_FP32 && impl != DFB_EDGE_IMPL_TC1) FAIL(ctx, DFB_E_INVALID, "unknown edge impl %d", impl);
+  if (impl != DFB_EDGE_IMPL_TC && impl != DFB_EDGE_IMPL_FP32 && impl != DFB_EDGE_IMPL_TC1 && impl != DFB_EDGE_IMPL_TC6)
+    FAIL(ctx, DFB_E_INVALID, "unknown edge impl %d", impl);
   ctx->edge_impl = impl;
   return DFB_OK;
 }
@@ -412,12 +413,16 @@ extern "C" int dfb_load_weights(dfb_ctx* ctx, int n_layers, int hidden_dim, int 
     size_t Wt_uvab, b_uvab, Wt_C, Wt_O, b_O, hg, hb, eg, eb, og, ob, Wt_tau, b_tau;
   };
   std::vector<LOff> lo(L);
-  std::vector<uint16_t> arena16((size_t)w_arena_rows(L) * H);
-  auto put16 = [&](const float* W, int row) {   // W [256 out][256 in] -> bf16 hi, lo at arena row `row`, K-major
+  std::vector<uint16_t> arena16((size_t)w_arena_rows(L) * H), arena16_3((size_t)w3_row(w_arena_rows(L)) * H);
+  // W [256 out][256 in] -> bf16 hi, lo at arena row `row`, K-major, and the third part bf16(W - hi - lo) at w3_row(row)
+  // of the third-part arena (W - hi and W - hi - lo are exact in fp32)
+  auto put16 = [&](const float* W, int row) {
     uint16_t* hi = &arena16[(size_t)row * H];
+    uint16_t* third = &arena16_3[(size_t)w3_row(row) * H];
     for (int i = 0; i < H * H; ++i) {
       hi[i] = f2bf16_rn(W[i]);
       hi[W_LO_ROWS * H + i] = f2bf16_rn(W[i] - bf16_to_f(hi[i]));
+      third[i] = f2bf16_rn(W[i] - bf16_to_f(hi[i]) - bf16_to_f(hi[W_LO_ROWS * H + i]));
     }
   };
   const float* p;
@@ -492,9 +497,11 @@ extern "C" int dfb_load_weights(dfb_ctx* ctx, int n_layers, int hidden_dim, int 
 
   ENS(ctx, ctx->wbuf, arena.size() * sizeof(float));
   ENS(ctx, ctx->wbuf16, arena16.size() * sizeof(uint16_t));
+  ENS(ctx, ctx->wbuf16_3, arena16_3.size() * sizeof(uint16_t));
   ENS(ctx, ctx->layers_dev, L * sizeof(LayerParams));
   CK(ctx, cudaMemcpy(ctx->wbuf.p, arena.data(), arena.size() * sizeof(float), cudaMemcpyHostToDevice));
   CK(ctx, cudaMemcpy(ctx->wbuf16.p, arena16.data(), arena16.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
+  CK(ctx, cudaMemcpy(ctx->wbuf16_3.p, arena16_3.data(), arena16_3.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
   const float* base = (const float*)ctx->wbuf.p;
   ctx->layers.resize(L);
   for (int l = 0; l < L; ++l) {
@@ -517,7 +524,7 @@ extern "C" int dfb_load_weights(dfb_ctx* ctx, int n_layers, int hidden_dim, int 
   ctx->lut = (float*)ctx->wbuf.p + o_lut;
   ctx->L = L; ctx->out_channels = out_channels; ctx->node_only = node_feature_only;
 
-  int r = tc_bind_weights(&ctx->tc, (const uint16_t*)ctx->wbuf16.p, L);
+  int r = tc_bind_weights(&ctx->tc, (const uint16_t*)ctx->wbuf16.p, (const uint16_t*)ctx->wbuf16_3.p, L);
   if (r) FAIL(ctx, DFB_E_CUDA, "tensor-map setup failed: %s", ctx->tc.err.c_str());
 
   // categorical edge-embedding LUT: edge_embed(edge_pos_embed(x)) for x in {0, 1}
@@ -720,10 +727,12 @@ extern "C" int dfb_prepare_graph_instances(dfb_ctx* ctx, const int64_t* edge_ind
 
 // What dfb_set_edge_impl selects for the linears and edge layers: the fp32 FFMA kernels (validation), or the
 // tensor-core kernels with nwg consumer warpgroups per edge-layer CTA (tc 2, tc1 1; under fp32 the GEMM1 dump of
-// dfb_debug_edge_gemm uses 2).
-struct EdgeImpl { bool fp32; int nwg; };
+// dfb_debug_edge_gemm uses 2) and npart bf16 parts per operand (tc6 3 on one warpgroup, for edge layers and linears
+// alike; the others 2).
+struct EdgeImpl { bool fp32; int nwg; int npart; };
 static EdgeImpl edge_impl(const dfb_ctx* ctx) {
-  return {ctx->edge_impl == DFB_EDGE_IMPL_FP32, ctx->edge_impl == DFB_EDGE_IMPL_TC1 ? 1 : 2};
+  const bool tc6 = ctx->edge_impl == DFB_EDGE_IMPL_TC6;
+  return {ctx->edge_impl == DFB_EDGE_IMPL_FP32, ctx->edge_impl == DFB_EDGE_IMPL_TC1 || tc6 ? 1 : 2, tc6 ? 3 : 2};
 }
 
 // rows X[R][256] -> Y = X W^T + b: fp32 FFMA (Wt in-major [256][N]) or the tensor-core linear (N / 256 matrices of the
@@ -736,7 +745,7 @@ static int linear_rows(dfb_ctx* ctx, const float* X, const float* Wt, int w_row,
     CKL(ctx);
     return DFB_OK;
   }
-  if (tc_launch_linear(&ctx->tc, X, Y, b, R, N / H, w_row, st))
+  if (tc_launch_linear(&ctx->tc, X, Y, b, R, N / H, w_row, edge_impl(ctx).npart, st))
     FAIL(ctx, DFB_E_CUDA, "tensor-core linear: %s", ctx->tc.err.c_str());
   ctx->launches++;
   return DFB_OK;
@@ -820,7 +829,7 @@ static int launch_edge_layer(dfb_ctx* ctx, int l, float* e, const float* uvab, c
   } else {
     if (tc_launch_edge_layer(&ctx->tc, l, e, uvab, (float*)ctx->partials.p, ctx->g, ctx->layers[l],
                              tvec_edge, tr, write_e, e_zero, xt_for_lut, ctx->lut, ctx->agg_mode, impl.nwg,
-                             ctx->phase_timing, nullptr, st))
+                             impl.npart, ctx->phase_timing, nullptr, st))
       FAIL(ctx, DFB_E_CUDA, "tensor-core edge layer: %s", ctx->tc.err.c_str());
     ctx->launches++;
   }
@@ -1270,7 +1279,7 @@ extern "C" int dfb_debug_edge_gemm(dfb_ctx* ctx, int layer, const float* e_in, f
   if (layer < 0 || layer >= ctx->L) FAIL(ctx, DFB_E_INVALID, "layer out of range");
   if (tc_launch_edge_layer(&ctx->tc, layer, const_cast<float*>(e_in), (const float*)ctx->uvab.p,
                            (float*)ctx->partials.p, ctx->g, ctx->layers[layer], nullptr, TimeRows{}, 0, 0, nullptr, ctx->lut, AGG_SUM,
-                           edge_impl(ctx).nwg, false, acc_out, st))
+                           edge_impl(ctx).nwg, edge_impl(ctx).npart, false, acc_out, st))
     FAIL(ctx, DFB_E_CUDA, "tensor-core edge layer: %s", ctx->tc.err.c_str());
   ctx->launches++;
   return DFB_OK;

@@ -22,7 +22,9 @@
 // copied into the dead operand area with cp.async once a GEMM has drained, so they wait on memory without registers.
 // Precision: every 256x256 product is evaluated as  a_hi*b_hi + a_lo*b_hi + a_hi*b_lo  with
 // a = a_hi + a_lo, b = b_hi + b_lo in bf16 and fp32 accumulation: ~2^-17 relative error per product, which keeps the
-// 1e-4 fp32 contract (single-pass TF32/BF16 does not: SURVEY D9).
+// 1e-4 fp32 contract (single-pass TF32/BF16 does not: SURVEY D9).  With NPART = 3 (DFB_EDGE_IMPL_TC6, one consumer
+// warpgroup) both operands are split into three bf16 parts, exact for fp32, and the six products of order <= 2 are
+// issued: the split for confident heads, whose softmax turns the bf16x3 logits' 2^-17 into p errors above 1e-4.
 // The same kernel in "linear mode" computes the node-side linears and the embedding linears (GEMM1 + bias only).
 #pragma once
 #include <cuda.h>
@@ -44,7 +46,6 @@ constexpr int TC_KCH = 32;                      // K elements per weight chunk =
 constexpr int TC_B_BYTES = 256 * TC_KCH * 2;    // one weight chunk [256 rows x 32 K] bf16 (hi or lo) = 16 KB
 static_assert(TC_KCH * 2 == 64, "weight chunk rows are one 64-byte swizzle row (tensor map, wgmma_desc_sw64)");
 constexpr int TC_A_CHUNK = WG_ROWS * 128;       // one operand chunk [64 rows x 64 K] bf16 (hi or lo)
-constexpr int TC_A_BYTES = 8 * TC_A_CHUNK;      // 4 K-chunks x (hi, lo) per warpgroup = 64 KB = [64][256] fp32 messages
 // Row loads a consumer thread issues in the conversion before it uses the first of them (memory-level parallelism),
 // sized so that they fit next to the 128 accumulator registers without spills: float4 row loads of 32
 constexpr int CONV_BATCH = 16;
@@ -62,14 +63,26 @@ __host__ __device__ constexpr int w_row_UVAB(int l) { return w_row_C(l) + 2 * W_
 __host__ __device__ constexpr int w_row_embed(int L, int which) { return L * W_LAYER_ROWS + which * W_MAT_ROWS; }   // 0 edge, 1 node
 __host__ __device__ constexpr int w_arena_rows(int L) { return w_row_embed(L, 2); }
 
-template <int NWG>
+// The third bf16 part of every matrix (DFB_EDGE_IMPL_TC6), bf16(W - hi - lo), in an arena of its own with one block of
+// 256 rows per matrix, in the order of the product arena: a matrix's third part lies at half the arena row of its hi
+// block (every hi block starts at a multiple of W_MAT_ROWS = 2 * 256 rows).
+__host__ __device__ constexpr int w3_row(int w_row) { return w_row / 2; }
+
+// NPART bf16 parts per operand: 2 is the bf16x3 product path (hi, lo: a_hi*b_hi + a_lo*b_hi + a_hi*b_lo); 3 is
+// DFB_EDGE_IMPL_TC6 (hi, mid, lo: the six products of order <= 2, see edge_layer_wg_body's gemm).
+template <int NWG, int NPART = 2>
 struct TcCfg {
   static_assert(NWG == 1 || NWG == 2, "one or two consumer warpgroups");
+  static_assert(NPART == 2 || NPART == 3, "two or three bf16 parts per operand");
   static constexpr int TILE = NWG * WG_ROWS;
   static constexpr int THREADS = (NWG + 1) * 128;
-  // one stage per weight chunk of a K block: hi K[0,32), hi K[32,64), lo K[0,32), lo K[32,64)
-  static constexpr int NSTAGE = 2 * TC_KBLK / TC_KCH;
-  static constexpr int OFF_B = NWG * TC_A_BYTES;
+  // one stage per weight chunk of a K block, part by part: hi K[0,32), hi K[32,64), lo K[0,32), lo K[32,64) (NPART 3:
+  // hi, mid, lo)
+  static constexpr int CPP = TC_KBLK / TC_KCH;   // weight chunks per part of a K block
+  static constexpr int NSTAGE = NPART * CPP;
+  static constexpr int A_BYTES = NPART * 4 * TC_A_CHUNK;   // a consumer warpgroup's A operand, NPART parts x 4 K blocks
+  static_assert(A_BYTES >= WG_ROWS * H * 4, "the [64][256] fp32 message rows fit in the A operand area");
+  static constexpr int OFF_B = NWG * A_BYTES;
   static constexpr int OFF_PRM = OFF_B + NSTAGE * TC_B_BYTES;   // ln_e_g, ln_e_b, tau, ln_o_g, ln_o_b, b_O
   static constexpr int OFF_ROW = OFF_PRM + 6 * H * 4;
   static constexpr int OFF_SRC = OFF_ROW + TILE * 4;
@@ -238,6 +251,20 @@ __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t&
   hi = *reinterpret_cast<uint32_t*>(&h);
   lo = *reinterpret_cast<uint32_t*>(&l);
 }
+// three-part forms (DFB_EDGE_IMPL_TC6): hi = rn(x), then the exact fp32 residual x - hi split into mid, lo as above
+__device__ __forceinline__ void split4(float4 x, uint2& hi, uint2& mid, uint2& lo) {
+  __nv_bfloat162 h01 = __floats2bfloat162_rn(x.x, x.y), h23 = __floats2bfloat162_rn(x.z, x.w);
+  float2 f01 = __bfloat1622float2(h01), f23 = __bfloat1622float2(h23);
+  hi.x = *reinterpret_cast<uint32_t*>(&h01);
+  hi.y = *reinterpret_cast<uint32_t*>(&h23);
+  split4(make_float4(x.x - f01.x, x.y - f01.y, x.z - f23.x, x.w - f23.y), mid, lo);
+}
+__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& mid, uint32_t& lo) {
+  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  const float2 f = __bfloat1622float2(h);
+  hi = *reinterpret_cast<uint32_t*>(&h);
+  split2(a - f.x, b - f.y, mid, lo);
+}
 // byte offset of (row r, 16-byte unit j in [0,8)) inside a [rows][64 bf16] K-major 128B-swizzled tile
 __device__ __forceinline__ uint32_t sw128_off(int r, int j) {
   return (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((j ^ (r & 7)) << 4));
@@ -295,9 +322,13 @@ enum {
 // ----------------------------------------------------------------------------------------------
 // LIN selects linear mode (k_linear_wg2); TIMED adds the phase timers (clock reads pin instruction order, so the product
 // entry points are built without); TROWS reads tau per row, through P.trows, instead of one vector for every row.
-template <int NWG, bool LIN, bool TIMED = false, bool TROWS = false>
-__device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, const TcParams& P) {
-  using Cfg = TcCfg<NWG>;
+// NPART 3 (DFB_EDGE_IMPL_TC6, NWG 1 only: three A parts of two warpgroups and a six-stage ring exceed shared memory)
+// stores A in three bf16 parts, streams each weight's third part from wmap3 as two more ring stages per K block and
+// issues six products per k16 step.
+template <int NWG, bool LIN, bool TIMED = false, bool TROWS = false, int NPART = 2>
+__device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, const TcParams& P,
+                                                   const CUtensorMap* wmap3 = nullptr) {
+  using Cfg = TcCfg<NWG, NPART>;
   constexpr int NSTAGE = Cfg::NSTAGE;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // stays in .shared
@@ -343,12 +374,15 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
           mbar_wait(&empty[s], ((u / NSTAGE) & 1) ^ 1, P.error_flag, 1);
           mbar_arrive_expect_tx(&full[s], TC_B_BYTES);
           // C, then O; linear mode: block (tile & 3) of U|V|A|B, or the one embedding.  Stage s of a K block holds the
-          // hi (s < NSTAGE / 2) or lo rows at K offset (s % (NSTAGE / 2)) * TC_KCH.
+          // hi (s < CPP) or lo rows at K offset (s % CPP) * TC_KCH; NPART 3: stages from 2 CPP on hold the third part.
           const int row = (lin ? P.lin_w_row + (P.lin_nb == 4 ? (tile & 3) : 0) * W_MAT_ROWS
                                : P.w_row_base + (i >= 4 * NSTAGE * NWG ? w_row_O(0) - w_row_C(0) : 0)) +
-                          (s >= NSTAGE / 2 ? W_LO_ROWS : 0);
-          const int k = ((i / NSTAGE) & 3) * TC_KBLK + (s % (NSTAGE / 2)) * TC_KCH;
-          tma_load_2d(smem_base + Cfg::OFF_B + s * TC_B_BYTES, &wmap, &full[s], k, row);
+                          (s >= Cfg::CPP ? W_LO_ROWS : 0);
+          const int k = ((i / NSTAGE) & 3) * TC_KBLK + (s % Cfg::CPP) * TC_KCH;
+          if (NPART == 3 && s >= 2 * Cfg::CPP)
+            tma_load_2d(smem_base + Cfg::OFF_B + s * TC_B_BYTES, wmap3, &full[s], k, w3_row(row - W_LO_ROWS));
+          else
+            tma_load_2d(smem_base + Cfg::OFF_B + s * TC_B_BYTES, &wmap, &full[s], k, row);
         }
       }
     }
@@ -360,8 +394,8 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
   const int wg = warp >> 2, wi = warp & 3, tid = threadIdx.x & 127;
   const int t4 = lane & 3;
   const int lr0 = wi * 16 + (lane >> 2);   // this thread's rows inside the warpgroup: lr0, lr0 + 8
-  unsigned char* a_reg = smem + wg * TC_A_BYTES;
-  const uint32_t a_base = smem_base + wg * TC_A_BYTES;
+  unsigned char* a_reg = smem + wg * Cfg::A_BYTES;
+  const uint32_t a_base = smem_base + wg * Cfg::A_BYTES;
   float* msg = reinterpret_cast<float*>(a_reg);   // [64][256] fp32, column c of row r at c ^ 8 (r & 7)
   int* w_row = s_row + wg * WG_ROWS;
   const float** w_src = s_src + wg * WG_ROWS;
@@ -405,6 +439,8 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
 
   // 4 K blocks x NSTAGE weight chunks against this warpgroup's A operand (hi, lo of K block kc at chunk 2 kc, 2 kc + 1).
   // Per K block: a_hi * b_hi and a_lo * b_hi for k16 steps 0..3 (the hi chunks), then a_hi * b_lo (the lo chunks).
+  // NPART 3 (A parts hi, mid, lo at chunks 3 kc .. 3 kc + 2; B parts hi, mid = the arena's lo, lo = the third part):
+  // every product of order <= 2, a_hi b_hi, a_mid b_hi, a_lo b_hi, then a_hi b_mid, a_mid b_mid, then a_hi b_lo.
   // Chunk s of K block kc sits in stage s, and this warpgroup's GEMMs take 4 NSTAGE ring positions each (so do the
   // other warpgroup's in between), so its full barrier completes its phase with parity kc & 1.  The stage stays a
   // compile-time constant: the K-block loop is rolled, the chunks inside it are not.
@@ -419,7 +455,7 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
     wgmma_fence();
 #pragma unroll 1
     for (int kc = 0; kc < 4; ++kc) {
-      const uint32_t ahi = a_base + kc * 2 * TC_A_CHUNK, alo = ahi + TC_A_CHUNK;
+      const uint32_t ahi = a_base + kc * NPART * TC_A_CHUNK, alo = ahi + TC_A_CHUNK, alo3 = alo + TC_A_CHUNK;
 #pragma unroll
       for (int s = 0; s < NSTAGE; ++s) {
         uint32_t w0 = 0;
@@ -427,14 +463,16 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
         mbar_wait(&full[s], kc & 1, P.error_flag, 2);
         if constexpr (TIMED) waited += (uint32_t)clock() - w0;
         const uint32_t b = smem_base + Cfg::OFF_B + s * TC_B_BYTES;
-        const bool b_hi = s < NSTAGE / 2;
+        const int pb = s / Cfg::CPP;   // B part of the chunk: 0 hi, 1 lo (NPART 3: mid), 2 lo
+        const bool b_hi = pb == 0;
 #pragma unroll
         for (int k = 0; k < TC_KCH / 16; ++k) {
-          const int ks = (s % (NSTAGE / 2)) * (TC_KCH / 16) + k;   // k16 step inside the K block
+          const int ks = (s % Cfg::CPP) * (TC_KCH / 16) + k;   // k16 step inside the K block
           const uint64_t db = wgmma_desc_sw64(b + k * 32);
           // hi*hi (B hi) or hi*lo (B lo); only the GEMM's very first wgmma overwrites acc
           wgmma_bf16(acc, wgmma_desc_sw128(ahi + ks * 32), db, (b_hi && ks == 0) ? (uint32_t)(kc != 0) : 1u);
-          if (b_hi) wgmma_bf16(acc, wgmma_desc_sw128(alo + ks * 32), db, 1u);   // lo*hi
+          if (pb + 1 < NPART) wgmma_bf16(acc, wgmma_desc_sw128(alo + ks * 32), db, 1u);    // lo*hi (NPART 3: mid*B)
+          if (pb + 2 < NPART) wgmma_bf16(acc, wgmma_desc_sw128(alo3 + ks * 32), db, 1u);   // NPART 3: lo*hi
         }
         wgmma_commit();
         wgmma_wait<1>();   // the previous chunk has been read (nothing to wait for at the GEMM's first)
@@ -493,7 +531,7 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
     }
     wg_bar();   // row table visible; every warp has left the previous tile's GEMM2 (A operand area free)
 
-    // ---------------- GEMM1 A operand: fp32 rows -> bf16 hi/lo, K-major 128B-swizzled chunks ----------------
+    // ---------------- GEMM1 A operand: fp32 rows -> bf16 hi/lo (NPART 3: hi/mid/lo), K-major 128B-swizzled chunks -----
     // CONV_BATCH row loads of a thread are issued before the first split: one memory round trip per batch.
 #pragma unroll 1
     for (int it0 = 0; it0 < 32; it0 += CONV_BATCH) {
@@ -507,11 +545,13 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
       for (int q = 0; q < CONV_BATCH; ++q) {
         const int item = (it0 + q) * 128 + tid;
         const int rr = item >> 6, k4 = item & 63;
-        uint2 hi, lo;
-        split4(x[q], hi, lo);
-        const uint32_t off = (k4 >> 4) * 2 * TC_A_CHUNK + sw128_off(rr, (k4 & 15) >> 1) + (k4 & 1) * 8;
+        uint2 hi, lo, lo3;   // NPART 3: hi, mid, lo
+        if constexpr (NPART == 2) split4(x[q], hi, lo);
+        else split4(x[q], hi, lo, lo3);
+        const uint32_t off = (k4 >> 4) * NPART * TC_A_CHUNK + sw128_off(rr, (k4 & 15) >> 1) + (k4 & 1) * 8;
         *reinterpret_cast<uint2*>(a_reg + off) = hi;
         *reinterpret_cast<uint2*>(a_reg + off + TC_A_CHUNK) = lo;
+        if constexpr (NPART == 3) *reinterpret_cast<uint2*>(a_reg + off + 2 * TC_A_CHUNK) = lo3;
       }
     }
     fence_proxy_async();   // generic-proxy stores -> visible to wgmma
@@ -665,11 +705,13 @@ __device__ __forceinline__ void edge_layer_wg_body(const CUtensorMap& wmap, cons
         const float2 b = *reinterpret_cast<const float2*>(prm + 4 * H + c);
         const float z0 = fmaf((acc[4 * j] - mean) * rstd, g.x, b.x);
         const float z1 = fmaf((acc[4 * j + 1] - mean) * rstd, g.y, b.y);
-        uint32_t hi, lo;
-        split2(z0 * sigmoid_mufu(z0), z1 * sigmoid_mufu(z1), hi, lo);   // SiLU
-        const uint32_t off = (j >> 3) * 2 * TC_A_CHUNK + sw128_off(r, j & 7) + 4 * t4;
+        uint32_t hi, lo, lo3;   // NPART 3: hi, mid, lo
+        if constexpr (NPART == 2) split2(z0 * sigmoid_mufu(z0), z1 * sigmoid_mufu(z1), hi, lo);   // SiLU
+        else split2(z0 * sigmoid_mufu(z0), z1 * sigmoid_mufu(z1), hi, lo, lo3);
+        const uint32_t off = (j >> 3) * NPART * TC_A_CHUNK + sw128_off(r, j & 7) + 4 * t4;
         *reinterpret_cast<uint32_t*>(a_reg + off) = hi;
         *reinterpret_cast<uint32_t*>(a_reg + off + TC_A_CHUNK) = lo;
+        if constexpr (NPART == 3) *reinterpret_cast<uint32_t*>(a_reg + off + 2 * TC_A_CHUNK) = lo3;
       }
       swap_row_halves(acc);
     }
@@ -741,6 +783,21 @@ __global__ void __launch_bounds__(TcCfg<2>::THREADS, 1)
 k_linear_wg2(const __grid_constant__ CUtensorMap wmap, const TcParams P) {
   edge_layer_wg_body<2, true>(wmap, P);
 }
+// DFB_EDGE_IMPL_TC6: the one-warpgroup body with three bf16 parts per operand, for the edge layers (with a timestep per
+// edge: _trows) and the linears.  wmap3 covers the third-part arena (w3_row).
+__global__ void __launch_bounds__(TcCfg<1, 3>::THREADS, 1)
+k_edge_layer_tc6(const __grid_constant__ CUtensorMap wmap, const __grid_constant__ CUtensorMap wmap3, const TcParams P) {
+  edge_layer_wg_body<1, false, false, false, 3>(wmap, P, &wmap3);
+}
+__global__ void __launch_bounds__(TcCfg<1, 3>::THREADS, 1)
+k_edge_layer_tc6_trows(const __grid_constant__ CUtensorMap wmap, const __grid_constant__ CUtensorMap wmap3,
+                       const TcParams P) {
+  edge_layer_wg_body<1, false, false, true, 3>(wmap, P, &wmap3);
+}
+__global__ void __launch_bounds__(TcCfg<1, 3>::THREADS, 1)
+k_linear_tc6(const __grid_constant__ CUtensorMap wmap, const __grid_constant__ CUtensorMap wmap3, const TcParams P) {
+  edge_layer_wg_body<1, true, false, false, 3>(wmap, P, &wmap3);
+}
 
 // ----------------------------------------------------------------------------------------------
 // host side
@@ -750,6 +807,7 @@ struct TcState {
   std::string err;
   int num_sms = 0;
   CUtensorMap wmap;
+  CUtensorMap wmap3;            // the third-part arena (DFB_EDGE_IMPL_TC6)
   bool bound = false;
   float* zero_row = nullptr;
   int* error_flag = nullptr;    // device alias of error_host (host-mapped: readable after a trap)
@@ -783,6 +841,13 @@ inline int tc_init(TcState* st, int num_sms) {
     e = cudaFuncSetAttribute(k_edge_layer_wg1_trows, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<1>::SMEM_ALLOC_TROWS);
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute(k_linear_wg2, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<2>::SMEM_ALLOC);
+  if (e == cudaSuccess)
+    e = cudaFuncSetAttribute(k_edge_layer_tc6, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<1, 3>::SMEM_ALLOC);
+  if (e == cudaSuccess)
+    e = cudaFuncSetAttribute(k_edge_layer_tc6_trows, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             TcCfg<1, 3>::SMEM_ALLOC_TROWS);
+  if (e == cudaSuccess)
+    e = cudaFuncSetAttribute(k_linear_tc6, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<1, 3>::SMEM_ALLOC);
   if (e != cudaSuccess) {
     st->err = std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e);
     return -2;
@@ -799,9 +864,10 @@ inline int tc_init(TcState* st, int num_sms) {
   return 0;
 }
 
-// One tensor map over the whole bf16 weight arena at `arena` (w_arena_rows(L) rows of 256 K, layout above).
-// Box = 32 K x 256 rows, 64-byte swizzle: one weight chunk.
-inline int tc_bind_weights(TcState* st, const uint16_t* arena, int L) {
+// One tensor map over the whole bf16 weight arena at `arena` (w_arena_rows(L) rows of 256 K, layout above), and one
+// over the third-part arena at `arena3` (w_arena_rows(L) / 2 rows, w3_row).  Box = 32 K x 256 rows, 64-byte swizzle:
+// one weight chunk.
+inline int tc_bind_weights(TcState* st, const uint16_t* arena, const uint16_t* arena3, int L) {
   void* fn = nullptr;
   cudaDriverEntryPointQueryResult qres;
   cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres);
@@ -810,49 +876,69 @@ inline int tc_bind_weights(TcState* st, const uint16_t* arena, int L) {
     cudaGetLastError();
     return -2;
   }
-  cuuint64_t gdim[2] = {(cuuint64_t)H, (cuuint64_t)w_arena_rows(L)};
+  st->bound = false;
   cuuint64_t gstride[1] = {(cuuint64_t)H * sizeof(uint16_t)};
   cuuint32_t box[2] = {(cuuint32_t)TC_KCH, 256u};
   cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = ((PFN_encodeTiled)fn)(&st->wmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)arena, gdim,
-                                     gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B,
-                                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    st->err = "cuTensorMapEncodeTiled failed with CUresult " + std::to_string((int)r);
-    return -2;
+  for (int m = 0; m < 2; ++m) {
+    cuuint64_t gdim[2] = {(cuuint64_t)H, (cuuint64_t)(m ? w3_row(w_arena_rows(L)) : w_arena_rows(L))};
+    CUresult r = ((PFN_encodeTiled)fn)(m ? &st->wmap3 : &st->wmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+                                       (void*)(m ? arena3 : arena), gdim, gstride, box, estr,
+                                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B,
+                                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+      st->err = "cuTensorMapEncodeTiled failed with CUresult " + std::to_string((int)r);
+      return -2;
+    }
   }
   st->bound = true;
   return 0;
 }
 
 // Launches `kernel` over tiles of TcCfg<NWG>::TILE rows of `rows` rows (times nb column blocks), persistent: one CTA
-// per SM, fewer when there are fewer tiles.  P holds the launch's own arguments; the context's are added here.
+// per SM, fewer when there are fewer tiles.  P holds the launch's own arguments; the context's are added here.  The
+// three-part kernels (DFB_EDGE_IMPL_TC6) take the third-part tensor map as well.
 template <int NWG>
-inline int tc_launch(TcState* st, void (*kernel)(CUtensorMap, TcParams), TcParams& P, int rows, int nb,
-                     cudaStream_t stream, int smem = TcCfg<NWG>::SMEM_ALLOC) {
+inline int tc_launch_prepare(TcState* st, TcParams& P, int rows, int nb) {
   if (!st->bound) {
     st->err = "weights not bound";
     return -1;
   }
   P.zero_row = st->zero_row; P.error_flag = st->error_flag; P.phase_cycles = st->phase_cycles;
   P.n_tiles = nb * ((rows + TcCfg<NWG>::TILE - 1) / TcCfg<NWG>::TILE);
-  const int grid = P.n_tiles < st->num_sms ? P.n_tiles : st->num_sms;
-  kernel<<<grid, TcCfg<NWG>::THREADS, smem, stream>>>(st->wmap, P);
+  return 0;
+}
+inline int tc_launch_done(TcState* st) {
   const cudaError_t err = cudaGetLastError();
   if (err == cudaSuccess) return 0;
   st->err = std::string("launch: ") + cudaGetErrorString(err);
   return -2;
 }
+template <int NWG>
+inline int tc_launch(TcState* st, void (*kernel)(CUtensorMap, TcParams), TcParams& P, int rows, int nb,
+                     cudaStream_t stream, int smem = TcCfg<NWG>::SMEM_ALLOC) {
+  if (int r = tc_launch_prepare<NWG>(st, P, rows, nb)) return r;
+  const int grid = P.n_tiles < st->num_sms ? P.n_tiles : st->num_sms;
+  kernel<<<grid, TcCfg<NWG>::THREADS, smem, stream>>>(st->wmap, P);
+  return tc_launch_done(st);
+}
+inline int tc_launch6(TcState* st, void (*kernel)(CUtensorMap, CUtensorMap, TcParams), TcParams& P, int rows, int nb,
+                      cudaStream_t stream, int smem = TcCfg<1, 3>::SMEM_ALLOC) {
+  if (int r = tc_launch_prepare<1>(st, P, rows, nb)) return r;
+  const int grid = P.n_tiles < st->num_sms ? P.n_tiles : st->num_sms;
+  kernel<<<grid, TcCfg<1, 3>::THREADS, smem, stream>>>(st->wmap, st->wmap3, P);
+  return tc_launch_done(st);
+}
 
 // One fused edge layer l over graph g.  nwg 2: k_edge_layer_wg2, the product kernel, or with `timed` its copy with
-// phase timers, k_edge_layer_wg2_timed; nwg 1: k_edge_layer_wg1, the 64-row-tile variant.  A non-null debug_acc
-// (tests) runs GEMM1 only and writes its accumulator [E][256] there, never through the timed copy.  With a non-null
-// trows.index (a TSP layer with a timestep per edge) the launch goes to k_edge_layer_wg<nwg>_trows, which has no
-// phase timers.
+// phase timers, k_edge_layer_wg2_timed; nwg 1: k_edge_layer_wg1, the 64-row-tile variant; npart 3 (DFB_EDGE_IMPL_TC6,
+// nwg ignored): k_edge_layer_tc6.  A non-null debug_acc (tests) runs GEMM1 only and writes its accumulator [E][256]
+// there, never through the timed copy.  With a non-null trows.index (a TSP layer with a timestep per edge) the launch
+// goes to k_edge_layer_wg<nwg>_trows (k_edge_layer_tc6_trows), which has no phase timers; neither has npart 3.
 inline int tc_launch_edge_layer(TcState* st, int l, float* e, const float* uvab, float* partials, const GraphDev& g,
                                 const LayerParams& lp, const float* tvec, const TimeRows& trows, int write_e,
-                                int e_zero, const float* xt_lut, const float* lut, int agg_mode, int nwg, bool timed,
-                                float* debug_acc, cudaStream_t stream) {
+                                int e_zero, const float* xt_lut, const float* lut, int agg_mode, int nwg, int npart,
+                                bool timed, float* debug_acc, cudaStream_t stream) {
   TcParams P{};
   P.e = e; P.uvab = uvab; P.partials = partials; P.g = g; P.lp = lp; P.tvec = tvec;
   P.xt_lut = xt_lut; P.lut = lut; P.debug_acc = debug_acc;
@@ -861,21 +947,25 @@ inline int tc_launch_edge_layer(TcState* st, int l, float* e, const float* uvab,
   P.w_row_base = w_row_C(l);
   if (trows.index && tvec && !debug_acc) {
     P.trows = trows;
+    if (npart == 3) return tc_launch6(st, k_edge_layer_tc6_trows, P, g.E, 1, stream, TcCfg<1, 3>::SMEM_ALLOC_TROWS);
     if (nwg == 1) return tc_launch<1>(st, k_edge_layer_wg1_trows, P, g.E, 1, stream, TcCfg<1>::SMEM_ALLOC_TROWS);
     return tc_launch<2>(st, k_edge_layer_wg2_trows, P, g.E, 1, stream, TcCfg<2>::SMEM_ALLOC_TROWS);
   }
+  if (npart == 3) return tc_launch6(st, k_edge_layer_tc6, P, g.E, 1, stream);
   if (nwg == 1) return tc_launch<1>(st, k_edge_layer_wg1, P, g.E, 1, stream);
   return tc_launch<2>(st, timed && !debug_acc ? k_edge_layer_wg2_timed : k_edge_layer_wg2, P, g.E, 1, stream);
 }
 
 // in [rows][256] times nb 256x256 matrices of the arena, the first at row w_row (w_row_*), -> out [rows][nb * 256]
-// + bias, on k_linear_wg2: the node linears U|V|A|B of a layer (nb 4) or an embedding linear (nb 1).
+// + bias, on k_linear_wg2 (npart 3: k_linear_tc6): the node linears U|V|A|B of a layer (nb 4) or an embedding linear
+// (nb 1).
 inline int tc_launch_linear(TcState* st, const float* in, float* out, const float* bias, int rows, int nb, int w_row,
-                            cudaStream_t stream) {
+                            int npart, cudaStream_t stream) {
   TcParams P{};
   P.lin_in = in; P.lin_out = out; P.lin_bias = bias; P.lin_rows = rows; P.lin_nb = nb; P.lin_w_row = w_row;
   // the kernel stages a layer's vectors in every mode; linear mode reads none of them
   P.lp.ln_e_g = P.lp.ln_e_b = P.lp.ln_o_g = P.lp.ln_o_b = P.lp.b_O = st->zero_row;
+  if (npart == 3) return tc_launch6(st, k_linear_tc6, P, rows, nb, stream);
   return tc_launch<2>(st, k_linear_wg2, P, rows, nb, stream);
 }
 

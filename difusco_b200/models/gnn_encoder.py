@@ -23,6 +23,10 @@ Interface notes (reference behaviour kept):
     [node_ptr[i], node_ptr[i+1])): one block-diagonal call over a ragged batch whose head GroupNorm
     runs per instance, so every instance gets the result it would get alone (the reference's test
     loader runs batch size 1).  Without it the GroupNorm statistics span every row of the call.
+  * edge_precision (keyword only, not in the reference) picks the tensor-core edge GEMMs' split: "bf16x3" (default,
+    three bf16 products) keeps the heat map within 1e-4 of the reference for logits of synthetic range; "bf16x6" (six
+    products of three-part operands, several times slower) keeps it there at any confidence, as a trained
+    checkpoint's heads need (include/difusco_b200.h, DFB_EDGE_IMPL_TC6).
 Only the forward is in scope: autograd is not supported - outputs carry no grad_fn, and a call with grad mode enabled
 on parameters that require grad warns once.  A training-step loss is evaluated under torch.no_grad().
 """
@@ -47,6 +51,9 @@ def reference_frequency_tables(hidden_dim):
   return {"__const.time_freqs": freqs.numpy(), "__const.dimt_pos": dimt_pos.numpy(),
           "__const.dimt_scalar": dimt_scalar.numpy()}
 
+
+# GNNEncoder(edge_precision=...) -> the edge implementation it selects
+EDGE_PRECISION = {"bf16x3": _cabi.EDGE_IMPL_TC, "bf16x6": _cabi.EDGE_IMPL_TC6}
 
 MAX_TIMESTEPS = 4096   # distinct timesteps of one call (the device step table of dfb_encoder_forward_timesteps)
 
@@ -120,8 +127,11 @@ class GNNEncoder(nn.Module):
   def __init__(self, n_layers, hidden_dim, out_channels=1, aggregation="sum", norm="layer",
                learn_norm=True, track_norm=False, gated=True,
                sparse=False, use_activation_checkpoint=False, node_feature_only=False,
-               *args, **kwargs):
+               *args, edge_precision="bf16x3", **kwargs):
     super().__init__()
+    if edge_precision not in EDGE_PRECISION:
+      raise ValueError(f"edge_precision must be one of {sorted(EDGE_PRECISION)}, got {edge_precision!r}")
+    self.edge_precision = edge_precision
     self.sparse = sparse
     self.node_feature_only = node_feature_only
     self.hidden_dim = hidden_dim
@@ -171,6 +181,7 @@ class GNNEncoder(nn.Module):
       self._ctx = _cabi.Context(idx)
       _cabi.device_context(idx, prefer=self._ctx)   # k-NN / 2-opt helpers share the first model's context
       self._ctx.set_aggregation(self.aggregation)
+      self._ctx.set_edge_impl(EDGE_PRECISION[self.edge_precision])
       self._weights_key = self._graph_key = self._points_key = None
     self._sync_weights()
     return self._ctx

@@ -92,6 +92,7 @@ class COMetaModel(_Base):
         sparse=self.sparse,
         use_activation_checkpoint=_arg(self.args, "use_activation_checkpoint", False),
         node_feature_only=node_feature_only,
+        edge_precision=_arg(self.args, "edge_precision", "bf16x3"),
     )
     self._step_counter = 0
 
